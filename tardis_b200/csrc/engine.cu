@@ -98,6 +98,7 @@ struct tb200_engine {
     int bulk_reps_used = 256;
     bool have_macro_guide = false;
     DBuf<unsigned long long> diff;  // jump algorithm: [S][lpad+1][4] fixed-point difference arrays
+    DBuf<unsigned long long> xfer;  // jump algorithm: [S-1][lpad+1][4] shell-crossing transfers, folded into diff per call
     double e_typ = 0.0;             // typical packet energy (sets the fixed-point scale)
     double diff_scale1 = 0.0, diff_scale2 = 0.0;  // scales of what the difference arrays hold (0 = they are empty)
     double finalize_ms = 0.0;
@@ -205,7 +206,7 @@ void tb200_destroy(tb200_engine *en) {
     cudaSetDevice(en->device);
     cudaStreamSynchronize(en->stream);
     en->r_inner.release(); en->r_outer.release(); en->n_e.release(); en->nu_line.release(); en->tau_t.release();
-    en->prefix.release(); en->first_le.release(); en->diff.release(); en->bulk_rep.release(); en->cnt_rep.release(); en->macro_guide.release(); en->tp_t.release(); en->grid.release(); en->staging.release();
+    en->prefix.release(); en->first_le.release(); en->diff.release(); en->xfer.release(); en->bulk_rep.release(); en->cnt_rep.release(); en->macro_guide.release(); en->tp_t.release(); en->grid.release(); en->staging.release();
     en->t_e.release(); en->bf_thr.release(); en->pi_min.release(); en->pi_max.release(); en->x_sect.release(); en->phot_nus.release();
     en->cb_B.release(); en->cb_mom.release(); en->cont_lit.release(); en->cb_guide.release(); en->cb_nact.release(); en->cb_pos.release(); en->cb_chi_lin.release();
     en->ff_factor.release(); en->chi_bf_t.release(); en->emiss_t.release(); en->markov_cum.release(); en->pi_refs.release(); en->pi_act.release();
@@ -676,10 +677,17 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
     if (en->opacity_pending) return fail(TB200_ERR_NO_MODEL, "the opacity tables are pending: tb200_set_model got no tau_sobolev, call tb200_build_opacity");
     CK(cudaSetDevice(en->device));
     const int S = en->S;
+    const size_t row_words = (size_t)(en->lpad + 1) * 4;  // one shell's row of the difference arrays
     if (first) {
+        if (en->algorithm == 1) {  // the transfers of one call start from zero whatever happens to diff
+            const size_t xfer_words = (size_t)(S > 1 ? S - 1 : 1) * row_words;
+            int rx = en->xfer.ensure(xfer_words);
+            if (rx) return rx;
+            CK(cudaMemsetAsync(en->xfer.p, 0, xfer_words * sizeof(unsigned long long), en->stream));
+        }
         if (zero_estimators) {
             CK(cudaMemsetAsync(en->est.p, 0, en->est_count * sizeof(double), en->stream));
-            if (en->algorithm == 1) CK(cudaMemsetAsync(en->diff.p, 0, (size_t)S * (en->lpad + 1) * 4 * sizeof(unsigned long long), en->stream));
+            if (en->algorithm == 1) CK(cudaMemsetAsync(en->diff.p, 0, (size_t)S * row_words * sizeof(unsigned long long), en->stream));
             if (en->continuum) {
                 CK(cudaMemsetAsync(en->cb_mom.p, 0, (size_t)S * (en->n_phot + 1) * tbc::N_MOMENTS * sizeof(double), en->stream));
                 CK(cudaMemsetAsync(en->cont_lit.p, 0, (size_t)5 * (en->n_continua > 0 ? en->n_continua : 1) * S * sizeof(double), en->stream));
@@ -772,7 +780,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         const double w2 = w1 / en->nu_typ;
         P.scale1 = ldexp(1.0, tb::FIXED_TYPICAL_LOG2 - ilogb(w1));
         P.scale2 = ldexp(1.0, tb::FIXED_TYPICAL_LOG2 - ilogb(w2));
-        P.diff = en->diff.p;
+        P.diff = en->diff.p; P.xfer = en->xfer.p;
         if (en->algorithm == 1) {
             // accumulating (zero_estimators == 0) into difference arrays that were filled at another scale would mix units
             if (first && zero_estimators) { en->diff_scale1 = 0.0; en->diff_scale2 = 0.0; }
@@ -893,6 +901,10 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         }
     }
     if (last && en->algorithm == 1) {
+        // diff[s] += xfer[s - 1] - xfer[s]: from here on diff holds every trace's +w / -w pair (trace_range_end)
+        tb::fold_transfers_kernel<<<(unsigned)((row_words / 2 + 255) / 256), 256, 0, en->stream>>>(en->diff.p, en->xfer.p, S, row_words);
+        en->launches++;
+        CK(cudaGetLastError());
         tb::finalize_line_estimators_kernel<<<2 * S, tb::FIN_THREADS, 0, en->stream>>>(en->diff.p, en->nu_line.p, en->L, en->lpad, 1.0 / P.scale1,
                                                                          1.0 / P.scale2, P.full_rel, P.jblue_t, P.edotlu_t, en->error.p);
         en->launches++;

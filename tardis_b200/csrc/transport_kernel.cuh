@@ -98,6 +98,8 @@ struct KParams {
     double *spec_emitted, *spec_reabsorbed;  // [n_grid - 1] fused energy histograms of the finished packets (or nullptr)
     // ---- jump algorithm: fixed-point difference arrays, [S][lpad+1][4] = {w1 hi, w1 lo, w2 hi, w2 lo} ----
     unsigned long long *diff;
+    unsigned long long *xfer;                // [S-1][lpad+1][4] transfers across the interface between shells s and s+1,
+                                             // folded into diff by fold_transfers_kernel (trace_range_end)
     double scale1, scale2;                   // powers of two
     // ---- scratch / control ----
     unsigned *rng_buf;                       // [n_warps][624][32]
@@ -361,17 +363,23 @@ __device__ __forceinline__ void red_u64(unsigned long long *addr, unsigned long 
 // spanning a factor 40 in frequency can produce) before the signed reading in finalize_line_estimators_kernel would be off
 // by 2^64 -- and that kernel notices: every trace adds +w at its first line and -w behind its last, so each row must sum to
 // exactly zero (ERR_FIXED_POINT otherwise).
+// fixed_term converts w once (false, with ERR_FIXED_POINT raised, when w * scale is out of range); fixed_add adds it or its
+// negative to one cell.
 constexpr double FIXED_SPLIT = 536870912.0;  // 2^29
 constexpr int FIXED_TYPICAL_LOG2 = 58;
-__device__ __forceinline__ void fixed_add(unsigned long long *cell, double w, double scale, bool negative, int *error) {
+struct FixedTerm { long long hi, lo; };
+__device__ __forceinline__ bool fixed_term(double w, double scale, FixedTerm &f, int *error) {
     const double t = w * scale;
     const double th = t * (1.0 / FIXED_SPLIT);
-    if (__builtin_expect(!(th < 4.0e18) || !(t >= 0.0), 0)) { atomicMax(error, ERR_FIXED_POINT); return; }
-    const long long hi = __double2ll_rd(th);
-    const long long lo = __double2ll_rn(t - (double)hi * FIXED_SPLIT);
+    if (__builtin_expect(!(th < 4.0e18) || !(t >= 0.0), 0)) { atomicMax(error, ERR_FIXED_POINT); return false; }
+    f.hi = __double2ll_rd(th);
+    f.lo = __double2ll_rn(t - (double)f.hi * FIXED_SPLIT);
+    return true;
+}
+__device__ __forceinline__ void fixed_add(unsigned long long *cell, const FixedTerm &f, bool negative) {
     if (cP.debug_skip_bulk & 2) return;  // experiments only
-    red_u64(cell, (unsigned long long)(negative ? -hi : hi));
-    red_u64(cell + 1, (unsigned long long)(negative ? -lo : lo));
+    red_u64(cell, (unsigned long long)(negative ? -f.hi : f.hi));
+    red_u64(cell + 1, (unsigned long long)(negative ? -f.lo : f.lo));
 }
 
 struct Counters {
@@ -460,6 +468,8 @@ struct Lane {
     int icount, bbuf;  // TrackerLastInteraction.interactions_count / _boundary_interactions_buffer
     int nev;           // rows written to the TrackerFull log
     int nsteps;        // events of this packet so far (watchdog)
+    int seg_open;      // jump kernels: the +w that opens this trace's estimator range was already added by the transfer at the
+                       // shell crossing that ended the previous trace (trace_range_end)
 };
 
 __device__ __noinline__ void log_boundary_slow(Lane &p, int from_shell, int to_shell) {
@@ -1236,7 +1246,7 @@ __device__ __noinline__ void start_packet_impl(Lane &p, Rng &rng, long long pid,
     const int L = P.n_lines;
     p.pid = (int)pid;
     p.r = P.in_r[pid]; p.mu = P.in_mu[pid]; p.nu = P.in_nu[pid]; p.energy = P.in_energy[pid];
-    p.shell = 0; p.status = ST_IN_PROCESS; p.icount = 0; p.bbuf = -1; p.nev = 0; p.nsteps = 0;
+    p.shell = 0; p.status = ST_IN_PROCESS; p.icount = 0; p.bbuf = -1; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
     rng.start(P.seed[pid], P.seed_x397[pid], (unsigned)pid);
     // set_packet_props_{partial,full}_relativity, modes/classic/packet_propagation.py:255-318
     double velocity = p.r / P.t_exp;
@@ -1598,7 +1608,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
     rng.start(0u, 0u, 0u);
     rng.ring = threadIdx.x & 31;
     Lane p;
-    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0;
+    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
     bool has = false;
     WarpFeed feed;
     Counters c;
@@ -1820,20 +1830,42 @@ struct TraceProbe {
     }
 };
 
-// lines [start, end) of shell get their estimators updated by this trace
+// Lines [start, end) of the packet's shell get their estimator updates from the trace that just ended: +w at start and -w
+// at end in the shell's difference row (w1 = E / nu, or E with full relativity; w2 = w1 / nu).  A packet that crosses into
+// a neighbouring shell keeps its weight (neither the move nor the crossing changes the lab-frame E and nu) and its next
+// range starts at the same column, so "-w at (s, end), +w at (s', end)" is ONE transfer: +w at xfer[s][end] for
+// s' = s + 1, -w at xfer[s - 1][end] for s' = s - 1; fold_transfers_kernel later adds xfer[s - 1] - xfer[s] to diff[s].
+// A range is opened at its start only when no transfer opened it (p.seg_open), and closed at its end only where the
+// weight or the row really ends: an interaction, or the packet leaving the grid.  An empty range that nothing opened adds
+// nothing; one that a transfer opened is transferred on or closed like any other (+w and -w at one cell cancel).  The
+// words are integers added mod 2^64, so the folded diff equals that of a direct +w / -w pair per trace bit for bit.
+// cross: +1 / -1 when the trace ends on an in-grid crossing into shell + cross, else 0.  end >= start.
 template <bool FR>
-__device__ __forceinline__ void range_update(const Lane &p, int start, int end, Counters &c) {
+__device__ __forceinline__ void trace_range_end(Lane &p, int start, int end, int cross, Counters &c) {
     const KParams &P = cP;
-    if (end <= start) return;
+    if (end <= start && !p.seg_open) return;
     c.line_steps += (unsigned long long)(end - start);
     const double inv_nu = 1.0 / p.nu;
     const double w1 = FR ? p.energy : p.energy * inv_nu;
     const double w2 = w1 * inv_nu;
-    unsigned long long *row = P.diff + (size_t)p.shell * (P.lpad + 1) * 4;
-    fixed_add(row + (size_t)start * 4, w1, P.scale1, false, P.error);
-    fixed_add(row + (size_t)start * 4 + 2, w2, P.scale2, false, P.error);
-    fixed_add(row + (size_t)end * 4, w1, P.scale1, true, P.error);
-    fixed_add(row + (size_t)end * 4 + 2, w2, P.scale2, true, P.error);
+    const size_t row_words = (size_t)(P.lpad + 1) * 4;
+    FixedTerm f;  // one term at a time, converted where it is added: the kernels sit at their register limit
+    if (!p.seg_open) {
+        unsigned long long *cell = P.diff + (size_t)p.shell * row_words + (size_t)start * 4;
+        if (fixed_term(w1, P.scale1, f, P.error)) fixed_add(cell, f, false);
+        if (fixed_term(w2, P.scale2, f, P.error)) fixed_add(cell + 2, f, false);
+    }
+    unsigned long long *cell = (cross != 0 ? P.xfer + (size_t)(p.shell - (cross < 0 ? 1 : 0)) * row_words
+                                           : P.diff + (size_t)p.shell * row_words) + (size_t)end * 4;
+    const bool negative = cross <= 0;
+    if (fixed_term(w1, P.scale1, f, P.error)) fixed_add(cell, f, negative);
+    if (fixed_term(w2, P.scale2, f, P.error)) fixed_add(cell + 2, f, negative);
+    p.seg_open = cross != 0;
+}
+
+// cross argument of trace_range_end for a trace that ends on the boundary towards shell + delta_shell
+__device__ __forceinline__ int grid_crossing(const Lane &p, int delta_shell) {
+    return (unsigned)(p.shell + delta_shell) < (unsigned)cP.n_shells ? delta_shell : 0;
 }
 
 // What a trace that did not end in the common fast way leaves behind for phase B.
@@ -1966,9 +1998,10 @@ __device__ __forceinline__ bool trace_phase_a(Lane &p, Rng &rng, Counters &c, do
             ps.state = 0;  // an interaction right at the guessed line
             return true;
         }
-        range_update<FR>(p, start, g, c);
+        trace_range_end<FR>(p, start, g, grid_crossing(p, t.delta_shell), c);
         p.next_line = g;
     }
+    // (start >= L: no range, and none is open -- transfers happen at columns <= L - 1 only, so seg_open implies start < L)
     if (CONT) trace_bf_estimators(p, t, t.d_boundary, s_ffh, c.bf_upd);
     move_and_bulk<FR>(p, t.d_boundary, s_J, s_nubar);
     boundary_event(p, t.delta_shell, c);
@@ -1984,7 +2017,7 @@ __device__ __forceinline__ void event_phase_b(Lane &p, Rng &rng, Counters &c, do
     const KParams &P = cP;
     const int L = P.n_lines;
     const int start = p.next_line;
-    int itype;
+    int itype, end = start;  // end of the estimator range (state 3, list exhausted: none)
     double distance;
     if (pk_state == 3) {
         itype = IT_ESCATTERING;
@@ -2017,12 +2050,14 @@ __device__ __forceinline__ void event_phase_b(Lane &p, Rng &rng, Counters &c, do
         }
         const int f = lo;
         itype = fb.p1 ? ((t.d_boundary <= fb.dcont) ? IT_BOUNDARY : IT_ESCATTERING) : IT_LINE;
-        range_update<FR>(p, start, fb.p1 ? f : f + 1, c);
+        end = fb.p1 ? f : f + 1;
         p.next_line = f;
         if (itype == IT_BOUNDARY) distance = t.d_boundary;
         else if (itype == IT_ESCATTERING) distance = (t.tau_event - fb.excl) / t.chi;
         else distance = distance_line_literal<FR>(p.r, p.mu, p.nu, t.comov_nu, false, P.nu_line[f], P.t_exp, P.error);
     }
+    // closed before the interaction changes the weight; a boundary crossing transfers it
+    trace_range_end<FR>(p, start, end, itype == IT_BOUNDARY ? grid_crossing(p, t.delta_shell) : 0, c);
     itype = resolve_continuum_type<CONT>(itype, t, rng);
     ev_type = itype;
     if (CONT) trace_bf_estimators(p, t, distance, s_ffh, c.bf_upd);
@@ -2060,7 +2095,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
     rng.start(0u, 0u, 0u);
     rng.ring = threadIdx.x & 31;
     Lane p;
-    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0;
+    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
     bool has = false, parked = false, vpend = false;
     WarpFeed feed;
     Counters c;
@@ -2142,12 +2177,12 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
 // with another runnable packet at once (taken from the same slot when that held a stashed runnable packet); once
 // park_min packets are parked the lanes swap their runnable packets against parked ones (which stashes the runnable
 // ones in the very same slots), handle the events, and carry on tracing with the packets they just handled.
-// A packet's trajectory does not depend on where it waits: its RNG state and ring id travel with it.
+// A packet's trajectory does not depend on where it waits: its RNG state, ring id and seg_open bit travel with it.
 // Pool slot = [POOL_ND doubles][POOL_NI ints], slot index fastest (conflict-free: lanes use distinct slots).
 // ------------------------------------------------------------------------------------------
 // (continuum mode: five more doubles {chi_bf_tot, chi_ff, escat_prob, dop, boltz} and two more ints {bin, active continua})
 __host__ __device__ constexpr int pool_nd(bool cont) { return cont ? 15 : 10; }
-__host__ __device__ constexpr int pool_ni(bool cont) { return cont ? 14 : 12; }
+__host__ __device__ constexpr int pool_ni(bool cont) { return cont ? 15 : 13; }
 __host__ __device__ constexpr int pool_bytes_per_slot(bool cont) { return pool_nd(cont) * 8 + pool_ni(cont) * 4 + 4; }  // + one int of the per-warp slot list
 
 template <bool CONT>
@@ -2158,11 +2193,13 @@ struct PoolView {
         d[s] = q.r; d[ns + s] = q.mu; d[2 * ns + s] = q.nu; d[3 * ns + s] = q.energy;
         i[s] = q.pid; i[ns + s] = q.next_line; i[2 * ns + s] = q.shell; i[3 * ns + s] = q.icount; i[4 * ns + s] = q.bbuf;
         i[5 * ns + s] = q.nev; i[6 * ns + s] = q.nsteps; i[7 * ns + s] = (int)r.n; i[8 * ns + s] = (int)r.a; i[9 * ns + s] = (int)r.b;
+        i[12 * ns + s] = q.seg_open;
     }
     __device__ __forceinline__ void get_packet(int s, Lane &q, Rng &r) const {
         q.r = d[s]; q.mu = d[ns + s]; q.nu = d[2 * ns + s]; q.energy = d[3 * ns + s];
         q.pid = i[s]; q.next_line = i[ns + s]; q.shell = i[2 * ns + s]; q.icount = i[3 * ns + s]; q.bbuf = i[4 * ns + s];
         q.nev = i[5 * ns + s]; q.nsteps = i[6 * ns + s]; r.n = (unsigned)i[7 * ns + s]; r.a = (unsigned)i[8 * ns + s]; r.b = (unsigned)i[9 * ns + s];
+        q.seg_open = i[12 * ns + s];
         q.status = ST_IN_PROCESS; r.pid = (unsigned)q.pid;
     }
     __device__ __forceinline__ void put_trace(int s, const ParkState &ps, unsigned ring) const {
@@ -2170,7 +2207,7 @@ struct PoolView {
         d[8 * ns + s] = ps.fb.excl; d[9 * ns + s] = ps.fb.dcont;
         if (CONT) {
             d[10 * ns + s] = ps.t.chi_bf_tot; d[11 * ns + s] = ps.t.chi_ff; d[12 * ns + s] = ps.t.escat_prob; d[13 * ns + s] = ps.t.dop;
-            d[14 * ns + s] = ps.t.boltz; i[12 * ns + s] = ps.t.cg; i[13 * ns + s] = ps.t.cn;
+            d[14 * ns + s] = ps.t.boltz; i[13 * ns + s] = ps.t.cg; i[14 * ns + s] = ps.t.cn;
         }
         i[10 * ns + s] = ps.g;
         i[11 * ns + s] = ps.state | (ps.fb.b ? 4 : 0) | (ps.fb.p1 ? 8 : 0) | ((ps.t.delta_shell + 1) << 4) | (int)(ring << 9);
@@ -2185,7 +2222,7 @@ struct PoolView {
         state = w & 3; fb.b = (w & 4) != 0; fb.p1 = (w & 8) != 0; t.delta_shell = ((w >> 4) & 3) - 1;
         if (CONT) {
             t.chi_bf_tot = d[10 * ns + s]; t.chi_ff = d[11 * ns + s]; t.escat_prob = d[12 * ns + s]; t.dop = d[13 * ns + s];
-            t.boltz = d[14 * ns + s]; t.cg = i[12 * ns + s]; t.cn = i[13 * ns + s];
+            t.boltz = d[14 * ns + s]; t.cg = i[13 * ns + s]; t.cn = i[14 * ns + s];
         } else { t.chi_bf_tot = 0.0; t.chi_ff = 0.0; t.escat_prob = 1.0; t.dop = 1.0; t.boltz = 0.0; t.cg = -1; t.cn = 0; }
     }
     // list[k] = index of the k-th set bit of `first`, then of `second` (both uniform across the warp)
@@ -2241,7 +2278,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_pool_kernel() {
     rng.start(0u, 0u, 0u);
     rng.ring = (unsigned)lane;
     Lane p;
-    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0;
+    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
     bool has = false;
     WarpFeed feed;
     Counters c;
@@ -2633,8 +2670,28 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_line_estimators_kernel(c
         carry += (__int128)(((unsigned __int128)tot_hi[31] << 64) | tot_lo[31]);
         __syncthreads();  // the totals are overwritten by the next tile
     }
-    // every range update is a +w / -w pair inside this row: a non-zero total means a 64-bit word wrapped (fixed_add)
-    if (threadIdx.x == 0 && carry != 0) atomicMax(error, ERR_FIXED_POINT);
+    // every range update is a +w / -w pair inside this row: a non-zero total means a 64-bit word wrapped (fixed_add).
+    // Unless an error already stopped the launch: the packets it was carrying keep the ranges that transfers opened
+    // (trace_range_end) unclosed, so the totals say nothing and the error that stopped it is the one to report.
+    if (threadIdx.x == 0 && carry != 0) atomicCAS(error, 0, ERR_FIXED_POINT);
+}
+
+// diff[s] += xfer[s - 1] - xfer[s] element-wise mod 2^64 (the transfers of trace_range_end; xfer has rows 0 .. S - 2).
+// One thread per 16 bytes of a row walks down the shells, so every transfer word is read once.
+__global__ void fold_transfers_kernel(unsigned long long *diff, const unsigned long long *xfer, int n_shells, size_t row_words) {
+    const size_t k = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
+    if (k >= row_words) return;
+    ulonglong2 below = make_ulonglong2(0ull, 0ull);  // xfer[s - 1]
+#pragma unroll 4
+    for (int s = 0; s < n_shells; s++) {
+        const ulonglong2 above = (s + 1 < n_shells) ? *reinterpret_cast<const ulonglong2 *>(xfer + (size_t)s * row_words + k)
+                                                    : make_ulonglong2(0ull, 0ull);
+        ulonglong2 *d = reinterpret_cast<ulonglong2 *>(diff + (size_t)s * row_words + k);
+        ulonglong2 v = *d;
+        v.x += below.x - above.x; v.y += below.y - above.y;
+        *d = v;
+        below = above;
+    }
 }
 
 // replicas {J | nu_bar | luminosity sums | ff_heating} -> packed estimator buffer (adds, then clears the replicas)
