@@ -335,6 +335,23 @@ __device__ __forceinline__ double distance_line_literal(double r, double mu, dou
     return (nu_diff / nu) * C_LIGHT * t_exp;
 }
 
+// Partial relativity inside the trace loops: the distance to a line as nu_diff * d_scale with d_scale = c t * (1 / nu),
+// computed once per trace, instead of the reference's (nu_diff / nu) * c * t.  The product carries four roundings
+// (1 / nu, c t, d_scale, the product), the reference's expression three, each <= u = 2^-53 relative, so the two differ
+// by at most ~7u = 8e-16 relative (4 ulps seen in practice) -- enough to decide `d_boundary <= d` the other way when
+// the line sits at the boundary.  Within PR_TIE_MARGIN = 1e-14 (> 12 x 7u) of d_boundary the reference's expression is
+// recomputed and decides (scan kernel); outside it both lie on the same side of d_boundary.  The jump kernels search with
+// the plain product and redo the search with the reference's expression when its result lies at such a tie
+// (trace_phase_a, event_phase_b): a check in every probe costs the pooled kernel ~4 %.
+// (The recomputation is out of line: it is rarely taken, and a division inlined at every call site bloats the hot loops.)
+constexpr double PR_TIE_MARGIN = 1e-14;
+__device__ __noinline__ double line_distance_partial_literal(double nu_diff, double nu) { return (nu_diff / nu) * C_LIGHT * cP.t_exp; }
+__device__ __forceinline__ double line_distance_partial(double nu_diff, double d_scale, double nu, double d_boundary) {
+    const double d = nu_diff * d_scale;
+    if (__builtin_expect(fabs(d - d_boundary) <= PR_TIE_MARGIN * d_boundary, 0)) return line_distance_partial_literal(nu_diff, nu);
+    return d;
+}
+
 __device__ __forceinline__ double shfl_d(double v, int src) { return __shfl_sync(FULL, v, src); }
 __device__ __forceinline__ double shfl_up_d(double v, int d) { return __shfl_up_sync(FULL, v, d); }
 
@@ -1700,7 +1717,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
                 } else {
                     if (valid && !(nu_diff >= 0)) atomicMax(P.error, ERR_NU_DIFF);
                     if (FR) d = distance_line_full_relativity(nu_l, b_nu, P.t_exp, b_r, b_mu);
-                    else d = nu_diff * d_scale;
+                    else d = line_distance_partial(nu_diff, d_scale, b_nu, b_db);
                 }
                 // inclusive warp prefix sum of tau
                 double incl = tau_l;
@@ -1806,28 +1823,37 @@ struct TraceProbe {
         extern __shared__ double s_bulk[];
         inv_chi = (FR || CONT) ? 1.0 / t.chi : s_bulk[3 * P.n_shells + p.shell];  // the same quotient, computed once per CTA
     }
-    // distance to line i as trace_packet sees it (homologous_rad_packet_transport.py:100-117)
+    // distance to line i as trace_packet sees it (homologous_rad_packet_transport.py:100-117).  In partial relativity
+    // the product nu_diff * d_scale, or with EXACT the reference's (nu_diff / nu) * c * t (see line_distance_partial).
+    template <bool EXACT = false>
     __device__ __forceinline__ double line_distance(int i, double nu_l) const {
         const double nu_diff = t.comov_nu - nu_l;
         if (i == L - 1) return MISS_DISTANCE;
         if (fabs(nu_diff) * inv_nu < CLOSE_LINE_THRESHOLD) return 0.0;
         if (FR) return distance_line_full_relativity(nu_l, p.nu, cP.t_exp, p.r, p.mu);
-        return nu_diff * d_scale;
+        return EXACT ? line_distance_partial_literal(nu_diff, p.nu) : nu_diff * d_scale;
+    }
+    // partial relativity: the product for line i lies within PR_TIE_MARGIN of d_boundary, where it may fall on the other
+    // side of it than the reference's expression
+    __device__ __forceinline__ bool near_boundary(int i) const {
+        return fabs(line_distance(i, cP.nu_line[i]) - t.d_boundary) <= PR_TIE_MARGIN * t.d_boundary;
     }
     // stopping predicate of trace_packet at line i (homologous_rad_packet_transport.py:100-151)
-    __device__ __forceinline__ Brk operator()(int i) const {
+    template <bool EXACT = false>
+    __device__ __forceinline__ Brk probe(int i) const {
         const KParams &P = cP;
         n_probes++;
         const double nu_l = P.nu_line[i];
         const double excl = dd_diff(prow[i], p_start);
         const double incl = dd_diff(prow[i + 1], p_start);
-        const double d = line_distance(i, nu_l);
+        const double d = line_distance<EXACT>(i, nu_l);
         const double d_cont = (t.tau_event - excl) * inv_chi;
         const bool p1 = (d != 0.0) && (fmin(t.d_boundary, d_cont) <= d);
         const bool p2 = !p1 && !P.disable_line && (incl + t.chi * d > t.tau_event);
         Brk r; r.b = p1 || p2; r.p1 = p1; r.excl = excl; r.dcont = d_cont;
         return r;
     }
+    __device__ __forceinline__ Brk operator()(int i) const { return probe<false>(i); }
 };
 
 // Lines [start, end) of the packet's shell get their estimator updates from the trace that just ended: +w at start and -w
@@ -1941,15 +1967,18 @@ __device__ __forceinline__ bool trace_phase_a(Lane &p, Rng &rng, Counters &c, do
         // the line index (tau >= 0; rounding is monotone).  This is exactly `brk(g).p1 && boundary wins && !brk(g-1).b`.
         bool fast;
         if (!FR) {
+            // With the plain products; a distance within PR_TIE_MARGIN of d_boundary, where the product may round to the
+            // other side of it than the reference's expression, leaves the fast path and the exact probes below decide.
             c.probes += 1;
             const double nu_g = P.nu_line[g], nu_m = P.nu_line[gm];
             const double E = dd_diff(brk.prow[g], brk.p_start);
-            const double d_g = brk.line_distance(g, nu_g);
+            const double d_g = brk.template line_distance<false>(g, nu_g);
             const double dcont_g = (t.tau_event - E) * brk.inv_chi;
-            fast = (d_g != 0.0) && (t.d_boundary <= d_g) && (t.d_boundary <= dcont_g);
+            const double tie = PR_TIE_MARGIN * t.d_boundary;
+            fast = (d_g != 0.0) && (t.d_boundary + tie < d_g) && (t.d_boundary <= dcont_g);
             if (g > start) {
-                const double d_m = brk.line_distance(gm, nu_m);
-                const bool p1m = (d_m != 0.0) && (t.d_boundary <= d_m);
+                const double d_m = brk.template line_distance<false>(gm, nu_m);
+                const bool p1m = (d_m != 0.0) && (t.d_boundary - tie <= d_m);
                 const bool p2m = !p1m && !P.disable_line && (E + t.chi * d_m > t.tau_event);
                 fast = fast && !p1m && !p2m;
             }
@@ -2048,7 +2077,20 @@ __device__ __forceinline__ void event_phase_b(Lane &p, Rng &rng, Counters &c, do
                 if (b.b) { hi = mid; fb = b; } else lo = mid + 1;
             }
         }
-        const int f = lo;
+        int f = lo;
+        // Partial relativity: the probes compare the product nu_diff * d_scale with d_boundary.  The reference's expression
+        // decides differently only for a line whose product lies within PR_TIE_MARGIN of d_boundary, and as the distance
+        // grows with the line index, such a line would be f or f - 1: search again with the reference's expression.
+        if (!FR && __builtin_expect(brk.near_boundary(f) || (f > start && brk.near_boundary(f - 1)), 0)) {
+            lo = start; hi = L - 1;  // line L-1 always stops a trace (MISS_DISTANCE)
+            fb = brk.template probe<true>(hi);
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                const Brk b = brk.template probe<true>(mid);
+                if (b.b) { hi = mid; fb = b; } else lo = mid + 1;
+            }
+            f = lo;
+        }
         itype = fb.p1 ? ((t.d_boundary <= fb.dcont) ? IT_BOUNDARY : IT_ESCATTERING) : IT_LINE;
         end = fb.p1 ? f : f + 1;
         p.next_line = f;
