@@ -348,9 +348,11 @@ int tb200_last_kernel_ms(tb200_engine *engine, double *ms);          /* CUDA-eve
 int tb200_get_counters(tb200_engine *engine, tb200_counters *counters);
 int64_t tb200_kernel_launches(tb200_engine *engine);                 /* kernels launched by this engine so far */
 /* Tuning only (no option changes a result): "algorithm" (1 jump, default; 0 scan), "pooled" (1: per-warp packet pool in the
- * classic mode), "ctas_per_sm" / "park_min" (0 = the measured best for the kernel that will run), "threads_per_cta" (256 | 128),
- * "refill_min", "sort_packets", "sort_bits", "pipeline_chunks", "pipeline_edges" (1, default: the first and the last packet
- * range of tb200_run are a quarter of the others, their copies being the ones no kernel hides). */
+ * classic mode), "ctas_per_sm" / "park_min" (0 = the measured best for the kernel that will run; each kernel is compiled for
+ * its default CTAs per SM, so another ctas_per_sm only sizes the grid, at most to what fits), "threads_per_cta" (256 | 128),
+ * "vol_min", "refill_min", "sort_packets", "sort_bits", "pipeline_chunks", "pipeline_edges" (1, default: the first and the last
+ * packet range of tb200_run are a quarter of the others, their copies being the ones no kernel hides), "keep_opacity_tables".
+ * Any other name is an error. */
 int tb200_set_option(tb200_engine *engine, const char *name, int64_t value);
 
 #ifdef __cplusplus

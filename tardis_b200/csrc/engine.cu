@@ -64,16 +64,11 @@ struct tb200_engine {
     // options
     int ctas_per_sm = 0, threads_per_cta = 256;  // 0 = the measured best for the kernel that will run (launch_range)
     int refill_min = 0;             // 0 = the measured best for the kernel that will run: pooled classic 12, others 8
-    int debug_skip_bulk = 0;
     int sort_packets = 1;           // process packets in order of initial frequency (L2 locality); results unchanged
     int sort_bits = 5;              // mantissa bits of the ordering key (coarse buckets)
     int park_min = 0;     // 0 = measured best: 32 for the pooled kernel, 16 with one packet per lane
     int algorithm = 1;  // 0 = scan (stream the line list), 1 = jump (prefix-table search + range updates; default)
-    int order_local = 1;  // ordering kernels: per-block shared-memory counters (0: one global atomic per packet)
-    int scan_tma = 0;     // experiment: streaming kernel stages nu_line / tau tiles with cp.async.bulk + mbarrier (classic mode)
-    int rng_store = -1;   // -1 = continuum mode only (tens of draws per packet): tier-1 MT19937 outputs go to the ring as they are drawn
     int vol_min = 24;     // warp-cooperative volleys start when this many lanes of a warp wait for one
-    int warp_volley = 1;  // jump with virtual packets: warp-cooperative volleys (0: every lane traces its own volley)
     int pooled = 1;     // jump, classic mode: packet pool per warp (transport_pool_kernel); 0 = one packet per lane
     cudaEvent_t ev_fin = nullptr;
     cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
@@ -240,8 +235,6 @@ int tb200_set_option(tb200_engine *en, const char *name, int64_t value) {
     if (k == "ctas_per_sm") { if (value < 0 || value > 16) return fail(TB200_ERR_INVALID, "ctas_per_sm out of range"); en->ctas_per_sm = (int)value; }
     else if (k == "threads_per_cta") { if (value != 128 && value != 256) return fail(TB200_ERR_INVALID, "threads_per_cta must be 128 or 256"); en->threads_per_cta = (int)value; }
     else if (k == "refill_min") { if (value < 0 || value > 32) return fail(TB200_ERR_INVALID, "refill_min must be in [0, 32]"); en->refill_min = (int)value; }
-    else if (k == "cont_smem") { /* removed: per-CTA shared-memory continuum estimators measured slower */ }
-    else if (k == "debug_skip_bulk") { en->debug_skip_bulk = (int)value; }  // experiments: bit 0 J/nu_bar, bit 1 range updates
     else if (k == "pipeline_edges") { en->pipeline_edges = value ? 1 : 0; }
     else if (k == "pipeline_chunks") { if (value < 1 || value > 64) return fail(TB200_ERR_INVALID, "pipeline_chunks must be in [1, 64]"); en->pipeline_chunks = (int)value; }
     else if (k == "sort_packets") { en->sort_packets = value ? 1 : 0; }
@@ -249,21 +242,21 @@ int tb200_set_option(tb200_engine *en, const char *name, int64_t value) {
     else if (k == "park_min") { if (value < 0 || value > 32) return fail(TB200_ERR_INVALID, "park_min must be in [1, 32]"); en->park_min = (int)value; }
     else if (k == "pooled") { en->pooled = value ? 1 : 0; }
     else if (k == "keep_opacity_tables") { en->keep_opacity_tables = value ? 1 : 0; }
-    else if (k == "warp_volley") { en->warp_volley = value ? 1 : 0; }
-    else if (k == "order_local") { en->order_local = value ? 1 : 0; }
-    else if (k == "scan_tma") { en->scan_tma = value ? 1 : 0; }
-    else if (k == "rng_store") { en->rng_store = value < 0 ? -1 : (value ? 1 : 0); }
     else if (k == "vol_min") { if (value < 1 || value > 32) return fail(TB200_ERR_INVALID, "vol_min must be in [1, 32]"); en->vol_min = (int)value; }
     else if (k == "algorithm") { if (value < 0 || value > 1) return fail(TB200_ERR_INVALID, "algorithm must be 0 (scan) or 1 (jump)"); en->algorithm = (int)value; }
     else return fail(TB200_ERR_INVALID, "unknown option " + k);
     return TB200_OK;
 }
 
+// Slack past the last row of the line-list tables (nu_line, tau, and every table upload_strided_table makes): kept until
+// every reader of them is known not to read past shells * pad.
+constexpr size_t TABLE_SLACK = 128;
+
 static int upload_strided_table(tb200_engine *en, const double *src, int64_t rows, int64_t shells, int64_t row_stride,
                                 int64_t shell_stride, int pad, DBuf<double> &dst) {
     // Stage the host view as it lies in memory: the smallest contiguous span covering it.
     int r;
-    if ((r = dst.ensure((size_t)shells * pad + tb::TMA_TILE))) return r;  // (+ one tile: bulk copies of the scan kernel may read past the last row)
+    if ((r = dst.ensure((size_t)shells * pad + TABLE_SLACK))) return r;
     if (rows == 0 || shells == 0) { CK(cudaMemsetAsync(dst.p, 0, (size_t)shells * pad * sizeof(double), en->stream)); return TB200_OK; }
     if (row_stride < 0 || shell_stride < 0) return fail(TB200_ERR_INVALID, "negative strides are not supported");
     size_t span = (size_t)(rows - 1) * row_stride + (size_t)(shells - 1) * shell_stride + 1;
@@ -335,18 +328,18 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     if (!(en->nu_typ > 0)) en->nu_typ = 1.0;
     int r;
     const int S = en->S, L = en->L;
-    if ((r = en->r_inner.ensure(S)) || (r = en->r_outer.ensure(S)) || (r = en->n_e.ensure(S)) || (r = en->nu_line.ensure(en->lpad + tb::TMA_TILE))) return r;
+    if ((r = en->r_inner.ensure(S)) || (r = en->r_outer.ensure(S)) || (r = en->n_e.ensure(S)) || (r = en->nu_line.ensure(en->lpad + TABLE_SLACK))) return r;
     CK(cudaMemcpyAsync(en->r_inner.p, m->r_inner, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->r_outer.p, m->r_outer, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->n_e.p, m->electron_density, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
-    CK(cudaMemsetAsync(en->nu_line.p, 0, (en->lpad + tb::TMA_TILE) * sizeof(double), en->stream));
+    CK(cudaMemsetAsync(en->nu_line.p, 0, (en->lpad + TABLE_SLACK) * sizeof(double), en->stream));
     CK(cudaMemcpyAsync(en->nu_line.p, m->line_list_nu, L * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     en->opacity_pending = false;
     if (m->tau_sobolev) {
         if ((r = upload_strided_table(en, m->tau_sobolev, L, S, m->tau_line_stride, m->tau_shell_stride, en->lpad, en->tau_t))) return r;
     } else {  // built on the device by tb200_build_opacity
-        if ((r = en->tau_t.ensure((size_t)S * en->lpad + tb::TMA_TILE))) return r;
-        CK(cudaMemsetAsync(en->tau_t.p, 0, ((size_t)S * en->lpad + tb::TMA_TILE) * sizeof(double), en->stream));
+        if ((r = en->tau_t.ensure((size_t)S * en->lpad + TABLE_SLACK))) return r;
+        CK(cudaMemsetAsync(en->tau_t.p, 0, ((size_t)S * en->lpad + TABLE_SLACK) * sizeof(double), en->stream));
         en->opacity_pending = true;
     }
     if (c->n_grid > 0) {
@@ -702,13 +695,13 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
     const int threads = en->threads_per_cta;
     const bool vpackets = !en->continuum && en->cfg.number_of_vpackets > 0;
     const bool want_pool = en->algorithm == 1 && en->pooled && !vpackets;
-    const bool warp_volley = en->algorithm == 1 && vpackets && en->warp_volley;
+    const bool warp_volley = en->algorithm == 1 && vpackets;
     // resident CTAs per SM (x 256 threads), measured with scripts/perf_probe.py on the bench model on an H100 SXM at a 400 W power
     // limit: the pooled classic kernel (2e7 packets) is fastest at 2 of 1-4, the pooled continuum kernel (4e6 packets, 50 shells)
     // at 2 rather than 3, and the warp-volley kernel of virtual packets (1e8 packets x 10) at 2 rather than 3 (3.73 vs 3.90 s;
     // at 3 or 4 CTAs it is held to 80 / 64 registers and spills, at 2 it has 128 and none).  The lane-resident jump kernel
-    // (option pooled = 0; 3 with continuum) and the scan kernel (3) are not re-measured on the H100.  The option ctas_per_sm
-    // overrides the choice.
+    // (option pooled = 0; 3 with continuum) and the scan kernel (3) are not re-measured on the H100.  Each kernel is compiled
+    // for its own count (__launch_bounds__, the dispatch below); the option ctas_per_sm only sizes the grid, at most to what fits.
     const int ctas_per_sm = en->ctas_per_sm > 0 ? en->ctas_per_sm : (en->algorithm == 1 ? (en->continuum ? (want_pool ? 2 : 3) : 2) : 3);
     const int grid = en->sm_count * ctas_per_sm;
     const size_t n_warps = (size_t)grid * (threads / 32);
@@ -764,9 +757,8 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         P.macro_guide = (en->have_macro_guide && !en->continuum) ? en->macro_guide.p : nullptr;
         P.bulk_rep = en->bulk_rep.p; P.bulk_reps = BULK_REPS;
     }
-    P.warp_volley = warp_volley ? 1 : 0; P.vol_min = en->vol_min;
-    P.rng_store = (en->continuum && en->rng_store != 0) ? 1 : 0;  // (only the continuum kernels' draw sites carry the store)
-    P.refill_min = en->refill_min > 0 ? en->refill_min : (pooled && !en->continuum ? 12 : 8); P.park_min = park_min; P.pool_slots = pool_slots; P.rng_units = rng_units; P.debug_skip_bulk = en->debug_skip_bulk;
+    P.vol_min = en->vol_min;
+    P.refill_min = en->refill_min > 0 ? en->refill_min : (pooled && !en->continuum ? 12 : 8); P.park_min = park_min; P.pool_slots = pool_slots; P.rng_units = rng_units;
     P.J = en->est.p + en->off_J; P.nubar = en->est.p + en->off_nubar; P.vhist = en->est.p + en->off_vhist;
     P.jblue_t = en->est.p + en->off_jblue; P.edotlu_t = en->est.p + en->off_edotlu;
     if (en->n_grid > 1) { P.spec_emitted = en->est.p + en->off_spec; P.spec_reabsorbed = P.spec_emitted + (en->n_grid - 1); }
@@ -803,7 +795,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
             CK(cudaMemsetAsync(en->order_hist.p, 0, (size_t)n_okeys * sizeof(unsigned), en->stream));
             tb::order_hist_kernel<<<(unsigned)((n + 256 * tb::ORDER_ITEMS - 1) / (256 * tb::ORDER_ITEMS)), 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p);
             tb::order_scan_kernel<<<1, 1024, 0, en->stream>>>(en->order_hist.p, n_okeys);
-            tb::order_scatter_kernel<<<(unsigned)((n + 256 * tb::ORDER_ITEMS - 1) / (256 * tb::ORDER_ITEMS)), 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p, en->order.p + off, en->order_local);
+            tb::order_scatter_kernel<<<(unsigned)((n + 256 * tb::ORDER_ITEMS - 1) / (256 * tb::ORDER_ITEMS)), 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p, en->order.p + off);
             en->launches += 3;
             CK(cudaGetLastError());
         }
@@ -825,19 +817,14 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         }
         size_t smem = (size_t)(en->algorithm == 1 ? 4 : 2) * S * sizeof(double);  // jump: [4 S] shell table; scan: J, nu_bar rows
         if (smem > 200 * 1024) return fail(TB200_ERR_INVALID, "too many shells for the shared-memory bulk estimators");
-        const bool scan_tma = en->algorithm == 0 && en->scan_tma && !en->continuum && !P.full_rel;
-        if (scan_tma) {  // two-stage tile ring + two mbarriers per warp
-            smem = (smem + 15) / 16 * 16;
-            P.park_off = (int)(smem / sizeof(double));
-            smem += (size_t)(threads / 32) * tb::tma_doubles_per_warp() * sizeof(double);
-        }
         if (pooled) {  // packet pools of the warps
             P.park_off = (int)(smem / sizeof(double));
             smem += (size_t)(threads / 32) * pool_slots * tb::pool_bytes_per_slot(en->continuum != 0);
         } else if (en->algorithm == 1) {
-            // parked-lane columns: [6 doubles][3 ints] (classic) or [11 doubles][5 ints] (continuum) per thread, ints padded to whole doubles
+            // parked-lane columns (tb::TraceColumns), one per thread
+            const bool cont = en->continuum != 0;
             P.park_off = (int)(smem / sizeof(double));
-            smem += (size_t)(en->continuum ? 14 : 8) * threads * sizeof(double);
+            smem += (size_t)(tb::trace_nd(cont) * sizeof(double) + tb::trace_ni(cont) * sizeof(int)) * threads;
             if (warp_volley) {  // item slots of the warp-cooperative virtual-packet volleys
                 P.vol_off = (int)(smem / sizeof(double));
                 smem += (size_t)(threads / 32) * tb::vol_doubles_per_warp(P.full_rel != 0) * sizeof(double);
@@ -854,30 +841,19 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
     } while (0)
         CK(cudaMemcpyToSymbolAsync(tb::cP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, en->stream));
         if (ev_a) CK(cudaEventRecord(ev_a, en->stream));
-        {
-            const int occ = ctas_per_sm * threads / 256;  // resident 256-thread-equivalents per SM the launch asks for
-            if (en->continuum && pooled) {  // IIP mode: full relativity always (modes/iip/packet_propagation.py:104,123)
-                if (occ >= 3) TB_LAUNCH((tb::transport_pool_kernel<true, 3, true>)); else TB_LAUNCH((tb::transport_pool_kernel<true, 2, true>));
-            } else if (en->continuum) {
-                if (en->algorithm == 1) { if (occ >= 3) TB_LAUNCH((tb::transport_jump_kernel<true, 3, true>)); else TB_LAUNCH((tb::transport_jump_kernel<true, 2, true>)); }
-                else { TB_LAUNCH((tb::transport_scan_kernel<true, 2, true>)); }
-            } else if (pooled) {
-                if (P.full_rel) { if (occ >= 4) TB_LAUNCH((tb::transport_pool_kernel<true, 4>)); else if (occ == 3) TB_LAUNCH((tb::transport_pool_kernel<true, 3>)); else TB_LAUNCH((tb::transport_pool_kernel<true, 2>)); }
-                else { if (occ >= 4) TB_LAUNCH((tb::transport_pool_kernel<false, 4>)); else if (occ == 3) TB_LAUNCH((tb::transport_pool_kernel<false, 3>)); else TB_LAUNCH((tb::transport_pool_kernel<false, 2>)); }
-            } else if (warp_volley) {  // virtual packets: warp-cooperative volleys, packet state in local memory (ESC)
-                if (P.full_rel) { if (occ >= 4) TB_LAUNCH((tb::transport_jump_kernel<true, 4, false, true, true>)); else if (occ == 3) TB_LAUNCH((tb::transport_jump_kernel<true, 3, false, true, true>)); else TB_LAUNCH((tb::transport_jump_kernel<true, 2, false, true, true>)); }
-                else { if (occ >= 4) TB_LAUNCH((tb::transport_jump_kernel<false, 4, false, true, true>)); else if (occ == 3) TB_LAUNCH((tb::transport_jump_kernel<false, 3, false, true, true>)); else TB_LAUNCH((tb::transport_jump_kernel<false, 2, false, true, true>)); }
-            } else if (en->algorithm == 1 && vpackets && occ >= 4) {  // option warp_volley = 0: every lane traces its own volleys (ESC)
-                if (P.full_rel) TB_LAUNCH((tb::transport_jump_kernel<true, 4, false, true>));
-                else TB_LAUNCH((tb::transport_jump_kernel<false, 4, false, true>));
-            } else if (en->algorithm == 1) {
-                if (P.full_rel) { if (occ >= 4) TB_LAUNCH((tb::transport_jump_kernel<true, 4, false>)); else if (occ == 3) TB_LAUNCH((tb::transport_jump_kernel<true, 3, false>)); else TB_LAUNCH((tb::transport_jump_kernel<true, 2, false>)); }
-                else { if (occ >= 4) TB_LAUNCH((tb::transport_jump_kernel<false, 4, false>)); else if (occ == 3) TB_LAUNCH((tb::transport_jump_kernel<false, 3, false>)); else TB_LAUNCH((tb::transport_jump_kernel<false, 2, false>)); }
-            } else {
-                if (P.full_rel) { if (occ >= 3) TB_LAUNCH((tb::transport_scan_kernel<true, 3, false>)); else TB_LAUNCH((tb::transport_scan_kernel<true, 2, false>)); }
-                else if (scan_tma) { if (occ >= 3) TB_LAUNCH((tb::transport_scan_kernel<false, 3, false, true>)); else TB_LAUNCH((tb::transport_scan_kernel<false, 2, false, true>)); }
-                else { if (occ >= 3) TB_LAUNCH((tb::transport_scan_kernel<false, 3, false>)); else TB_LAUNCH((tb::transport_scan_kernel<false, 2, false>)); }
-            }
+        // one kernel per mode, compiled for the CTAs per SM its default runs at (see ctas_per_sm above)
+        if (en->continuum) {  // IIP mode: full relativity always (modes/iip/packet_propagation.py:104,123)
+            if (pooled) TB_LAUNCH((tb::transport_pool_kernel<true, 2, true>));
+            else if (en->algorithm == 1) TB_LAUNCH((tb::transport_jump_kernel<true, 3, true>));
+            else TB_LAUNCH((tb::transport_scan_kernel<true, 2, true>));
+        } else if (en->algorithm == 0) {
+            if (P.full_rel) TB_LAUNCH((tb::transport_scan_kernel<true, 3, false>)); else TB_LAUNCH((tb::transport_scan_kernel<false, 3, false>));
+        } else if (pooled) {
+            if (P.full_rel) TB_LAUNCH((tb::transport_pool_kernel<true, 2>)); else TB_LAUNCH((tb::transport_pool_kernel<false, 2>));
+        } else if (warp_volley) {  // virtual packets: warp-cooperative volleys
+            if (P.full_rel) TB_LAUNCH((tb::transport_jump_kernel<true, 2, false, true>)); else TB_LAUNCH((tb::transport_jump_kernel<false, 2, false, true>));
+        } else {  // option pooled = 0, or the pools do not fit
+            if (P.full_rel) TB_LAUNCH((tb::transport_jump_kernel<true, 2, false>)); else TB_LAUNCH((tb::transport_jump_kernel<false, 2, false>));
         }
 #undef TB_LAUNCH
         en->launches++;

@@ -90,8 +90,7 @@ struct KParams {
     const unsigned *seed, *seed_x397;
     const int *order;                        // optional processing order (packet ids), or nullptr
     int refill_min;                          // refill a warp when this many lanes are free
-    int debug_skip_bulk;                     // experiments only: bit 0 do not accumulate J / nu_bar, bit 1 no range updates
-    int park_min;                            // jump kernel: run the slow phase when this many lanes are parked
+    int park_min;                           // jump kernel: run the slow phase when this many lanes are parked
     double *out_nu, *out_energy;
     // ---- estimators (device, packed buffer) ----
     double *J, *nubar, *vhist, *jblue_t, *edotlu_t;
@@ -112,10 +111,7 @@ struct KParams {
     double *bulk_rep;                        // [bulk_reps][rep_stride] replicas {J(S) | nu_bar(S) | luminosity sums(4) | ff_heating(S, continuum)}
     int bulk_reps;                           // power of two
     int rep_stride;
-    int rng_store;                           // 1: every packet writes its MT19937 outputs 0..226 to its ring as it draws them (modes with
-                                             //    many draws per packet: no replay when output 227 is reached); 0: replay on demand
-    int warp_volley;                         // 1: the kernel runs the virtual-packet volleys warp-cooperatively (warp_volley); the
-    int vol_off, vol_min;                    //    per-lane volley calls are skipped.  vol_off: first double of the item area in smem;
+    int vol_off, vol_min;                    // warp-cooperative volleys: vol_off: first double of the item area in smem;
                                              //    vol_min: run the volleys when this many lanes wait for one
     double lum_nu_start, lum_nu_end;         // calculate_filtered_luminosity window (spectrum/luminosity.py:5-29), strict on both sides
     int park_off;                            // jump kernels: first double of the parked-packet area in dynamic shared memory
@@ -167,7 +163,7 @@ __device__ __noinline__ uint2 rng_slow_next(unsigned n, unsigned a, unsigned pid
     const unsigned st = (unsigned)cP.rng_units;
     unsigned *rg = cP.rng_buf + gwarp * (size_t)MT_N * st + ring;  // word k of this packet's ring at rg[k * st]
     unsigned xn, xn1, xm, k;
-    if (n == 227u && !cP.rng_store) rng_replay_tier1(cP.seed[pid], cP.seed_x397[pid], rg, st);
+    if (n == 227u && !cP.continuum) rng_replay_tier1(cP.seed[pid], cP.seed_x397[pid], rg, st);
     if (n < 624u) {
         k = n; xn = a;
         if (n < 623u) { xn1 = mt_init_next(a, n + 1u); a = xn1; } else { xn1 = rg[0]; }
@@ -199,7 +195,7 @@ __device__ __noinline__ uint4 rng_draw_pair(unsigned n, unsigned a, unsigned b, 
             a = xn1; b = mt_init_next(b, n + 398u);
             const unsigned y = (xn & 0x80000000u) | (xn1 & 0x7fffffffu);
             v = xm ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-            if (cP.rng_store) {
+            if (cP.continuum) {  // tier-1 words go to the ring as they are drawn: output 227 then needs no replay
                 const size_t gwarp = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
                 cP.rng_buf[(gwarp * (size_t)MT_N + n) * (unsigned)cP.rng_units + ring] = v;
             }
@@ -234,8 +230,8 @@ struct Rng {
         v ^= v >> 11; v ^= (v << 7) & 0x9d2c5680u; v ^= (v << 15) & 0xefc60000u; v ^= v >> 18;
         return v;
     }
-    // STORE = continuum-mode call site (tens of draws per packet): the out-of-line copy, which with the engine flag rng_store
-    // also writes every tier-1 word to the packet's ring as it is drawn, so that reaching output 227 needs no replay.  The
+    // STORE = continuum-mode call site (tens of draws per packet): the out-of-line copy, which in continuum mode also writes
+    // every tier-1 word to the packet's ring as it is drawn, so that reaching output 227 needs no replay.  The
     // classic kernels' call sites inline the draw and carry none of that (it slows the headline kernel down).
     template <bool STORE = false>
     __device__ __forceinline__ double next_double() {
@@ -394,7 +390,6 @@ __device__ __forceinline__ bool fixed_term(double w, double scale, FixedTerm &f,
     return true;
 }
 __device__ __forceinline__ void fixed_add(unsigned long long *cell, const FixedTerm &f, bool negative) {
-    if (cP.debug_skip_bulk & 2) return;  // experiments only
     red_u64(cell, (unsigned long long)(negative ? -f.hi : f.hi));
     red_u64(cell + 1, (unsigned long long)(negative ? -f.lo : f.lo));
 }
@@ -448,11 +443,11 @@ __device__ __forceinline__ int first_line_below(double nu) {
     return lo;
 }
 
-// first index with nu_line <= nu (guess helper; clamped by the callers)
 // (out of line: faster for the classic kernels' packet start and virtual-packet literal walk, slower at the continuum
 //  emission sites)
 __device__ __noinline__ int first_line_below_call(double nu) { return first_line_below(nu); }
 
+// first index with nu_line <= nu, L - 1 when there is none or nu is not positive (guess helper; clamped by the callers)
 __device__ __forceinline__ int first_line_at_or_below(double nu) {
     const KParams &P = cP;
     const int L = P.n_lines;
@@ -462,8 +457,9 @@ __device__ __forceinline__ int first_line_at_or_below(double nu) {
     if (kb < 0) return L - 1;
     int glo = P.nu_first_le[kb];
     int ghi = (kb > 0) ? P.nu_first_le[kb - 1] : L;
-    if (ghi - glo <= 8) {
-        int cnt = 0;
+    if (ghi - glo <= 8) {  // a bucket holds ~2 lines on average: eight independent loads, no dependent chain
+        // (a lane that needs the bisection below holds up its whole warp: with <= 4 that was 7 % of the traces)
+        int cnt = 0;  // number of bracket entries that are still > nu (the list is sorted; rows are padded)
 #pragma unroll
         for (int k = 0; k < 8; k++) cnt += (glo + k < ghi && P.nu_line[glo + k] > nu);
         return glo + cnt;
@@ -488,6 +484,13 @@ struct Lane {
     int seg_open;      // jump kernels: the +w that opens this trace's estimator range was already added by the transfer at the
                        // shell crossing that ended the previous trace (trace_range_end)
 };
+
+// the state of a lane that holds no packet yet
+__device__ __forceinline__ Lane idle_lane() {
+    Lane p;
+    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
+    return p;
+}
 
 __device__ __noinline__ void log_boundary_slow(Lane &p, int from_shell, int to_shell) {
     const KParams &P = cP;
@@ -999,7 +1002,7 @@ template <bool FR> __device__ __forceinline__ VpacketStart vpacket_start(const L
     return s;
 }
 
-// Per-lane volley (scan kernel; jump kernel with option warp_volley = 0): every lane traces the volley of its own packet.
+// Per-lane volley (scan kernel): every lane traces the volley of its own packet.
 template <bool FR>
 __device__ __noinline__ void vpacket_volley(const Lane &p, Rng &rng, unsigned long long &n_vp, unsigned long long &n_vsteps) {
     const KParams &P = cP;
@@ -1255,8 +1258,9 @@ __device__ __noinline__ void warp_volley(bool active, const Lane &p, Rng &rng, u
 
 // make_r_packet (modes/montecarlo_transport.py:41-66) + the prologue of packet_propagation
 // (modes/classic/packet_propagation.py:99-122)
-// VP = false: the caller never runs with virtual packets (continuum mode; the pooled kernels) -- their code, and the registers
-// the call to it would clobber, stay out of that kernel
+// VP = true: the caller traces virtual packets per lane (classic scan kernel).  VP = false (continuum mode; the jump kernels,
+// which run theirs warp-cooperatively or not at all): that code, and the registers the call to it would clobber, stay out
+// of the kernel
 template <bool FR, bool VP = true>
 __device__ __noinline__ void start_packet_impl(Lane &p, Rng &rng, long long pid, Counters &c) {
     const KParams &P = cP;
@@ -1289,7 +1293,7 @@ __device__ __noinline__ void start_packet_impl(Lane &p, Rng &rng, long long pid,
         P.last_before_energy[pid] = qnan; P.last_after_nu[pid] = qnan; P.last_after_mu[pid] = qnan;
         P.last_after_energy[pid] = qnan;
     }
-    if (VP && P.n_vpackets > 0 && !P.warp_volley) vpacket_volley<FR>(p, rng, c.vp, c.vsteps);  // packet_propagation.py:109-118
+    if (VP && P.n_vpackets > 0) vpacket_volley<FR>(p, rng, c.vp, c.vsteps);  // packet_propagation.py:109-118
     log_boundary(p, -1, 0);                                             // :120-122
     c.boundary++;
 }
@@ -1324,14 +1328,12 @@ __device__ __forceinline__ void move_and_bulk(Lane &p, double distance, double *
         double cen = p.energy * dop;
         double dd = distance;
         if (FR) dd *= dop;
-        if (!(P.debug_skip_bulk & 1)) {
-            if (SMEM) {  // scan kernel: per-CTA rows in shared memory
-                atomicAdd(&s_J[p.shell], cen * dd);
-                atomicAdd(&s_nubar[p.shell], cen * dd * cnu);
-            } else {     // jump kernels: global replicas (bulk_replica)
-                red_f64(&s_J[p.shell], cen * dd);
-                red_f64(&s_nubar[p.shell], cen * dd * cnu);
-            }
+        if (SMEM) {  // scan kernel: per-CTA rows in shared memory
+            atomicAdd(&s_J[p.shell], cen * dd);
+            atomicAdd(&s_nubar[p.shell], cen * dd * cnu);
+        } else {     // jump kernels: global replicas (bulk_replica)
+            red_f64(&s_J[p.shell], cen * dd);
+            red_f64(&s_nubar[p.shell], cen * dd * cnu);
         }
     }
 }
@@ -1384,7 +1386,7 @@ __device__ __noinline__ void interaction_event_impl(Lane &p, Rng &rng, int itype
         log_interaction_after(p, IT_ESCATTERING);
         c.escat_ev++;
     }
-    if (VP && P.n_vpackets > 0 && !P.warp_volley) vpacket_volley<FR>(p, rng, c.vp, c.vsteps);  // (VP: see start_packet_impl)
+    if (VP && P.n_vpackets > 0) vpacket_volley<FR>(p, rng, c.vp, c.vsteps);  // (VP: see start_packet_impl)
 }
 template <bool FR, bool CONT, bool VP = !CONT>
 __device__ __forceinline__ void interaction_event(Lane &p, Rng &rng, int itype, Counters &c) {
@@ -1411,10 +1413,8 @@ __device__ __forceinline__ void finish_packet(Lane &p, const Rng &rng, Counters 
         // Simulation.iterate's calculate_filtered_luminosity of the emitted / reabsorbed packets (simulation/base.py:455-466,
         // spectrum/luminosity.py:5-29; x 1 / time_of_simulation on the host): {emitted, emitted in window, reabsorbed, reabsorbed in window}
         double *lum = bulk_replica() + 2 * P.n_shells + (p.status == ST_EMITTED ? 0 : 2);
-        if (!(P.debug_skip_bulk & 4)) {  // (bit 2: experiments only)
-            red_f64(lum, p.energy);
-            if (p.nu > P.lum_nu_start && p.nu < P.lum_nu_end) red_f64(lum + 1, p.energy);
-        }
+        red_f64(lum, p.energy);
+        if (p.nu > P.lum_nu_start && p.nu < P.lum_nu_end) red_f64(lum + 1, p.energy);
     }
     if (P.spec_emitted && p.status != ST_ADIABATIC_COOLING) {
         // numpy.histogram(nu, bins=grid, weights=energy): bin i covers [grid[i], grid[i+1]), the last bin is closed
@@ -1496,6 +1496,22 @@ struct TraceSetup {
     int delta_shell;
     int cg, cn;                                         // continuum mode only: ContTrace {g, n_active}
 };
+// the continuum-mode fields as a classic-mode trace leaves them (trace_setup sets them in continuum mode)
+__device__ __forceinline__ void clear_continuum_fields(TraceSetup &t) {
+    t.chi_bf_tot = 0.0; t.chi_ff = 0.0; t.escat_prob = 1.0; t.dop = 1.0; t.boltz = 0.0; t.cg = -1; t.cn = 0;
+}
+
+// [4 S] shell table at the head of the jump kernels' dynamic shared memory {r_inner, r_outer, chi_e, 1 / chi_e} (see
+// trace_setup).  The caller synchronises the CTA before reading it.
+__device__ __forceinline__ void load_shell_table() {
+    const KParams &P = cP;
+    extern __shared__ double s_bulk[];
+    for (int i = threadIdx.x; i < P.n_shells; i += blockDim.x) {
+        const double chi_e = P.n_e[i] * P.sigma_thomson;
+        s_bulk[i] = P.r_inner[i]; s_bulk[P.n_shells + i] = P.r_outer[i];
+        s_bulk[2 * P.n_shells + i] = chi_e; s_bulk[3 * P.n_shells + i] = 1.0 / chi_e;
+    }
+}
 // GEO (jump kernels): shell radii and the electron-scattering opacity come from the [4][S] table the kernel copied to
 // the head of dynamic shared memory {r_inner, r_outer, chi_e, 1 / chi_e} -- they start the dependent chain of every
 // trace, and the L1 (31 % hit rate under this access pattern) does not keep even 20-entry arrays resident.
@@ -1545,77 +1561,13 @@ __device__ __forceinline__ int resolve_continuum_type(int itype, const TraceSetu
 }
 
 // ------------------------------------------------------------------------------------------
-// TMA staging for the streaming kernel (experiment, engine option "scan_tma"; DESIGN.md §3 records the outcome): instead of
-// every lane loading its entry of the next 32-line chunk with LDG, one lane issues bulk copies (cp.async.bulk, 1-D TMA) of
-// TMA_TILE-entry tiles of nu_line and of the shell's tau row into a two-stage shared-memory ring per warp; an mbarrier
-// per stage counts the bytes in.
-// ------------------------------------------------------------------------------------------
-constexpr int TMA_TILE = 128;  // entries per tile (1 KB per array)
-__host__ __device__ constexpr int tma_doubles_per_warp() { return 4 * TMA_TILE + 2; }  // {nu, tau} x 2 stages + 2 mbarriers
-__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_1d(void *dst, const void *src, unsigned bytes, unsigned long long *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(unsigned long long *bar, unsigned parity) {
-    unsigned ok;
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(ok)
-                 : "r"(smem_u32(bar)), "r"(parity)
-                 : "memory");
-    return ok != 0;
-}
-struct TmaRing {
-    double *wb;               // {nu stage 0, nu stage 1, tau stage 0, tau stage 1} x TMA_TILE doubles (pointer arithmetic, not an
-                              // array of pointers: indexing one with the stage would put the struct in local memory)
-    unsigned long long *bar;  // [2]
-    __device__ __forceinline__ double *nu(int s) const { return wb + s * TMA_TILE; }
-    __device__ __forceinline__ double *tau(int s) const { return wb + (2 + s) * TMA_TILE; }
-    unsigned phase;           // bit s: parity the next wait on stage s looks for
-    unsigned pending;         // bit s: a tile is on its way into stage s (warp-uniform)
-    __device__ __forceinline__ void issue(int s, const double *nu_src, const double *tau_src, int lane) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the generic-proxy reads of this stage are done (WAR)
-        if (lane == 0) {
-            mbar_expect_tx(bar + s, 2u * TMA_TILE * 8u);
-            tma_load_1d(nu(s), nu_src, TMA_TILE * 8u, bar + s);
-            tma_load_1d(tau(s), tau_src, TMA_TILE * 8u, bar + s);
-        }
-        pending |= 1u << s;
-    }
-    __device__ __forceinline__ void wait(int s, int *error) {
-        unsigned spins = 0;
-        while (!mbar_try_wait(bar + s, (phase >> s) & 1u)) {
-            if (++spins > (1u << 28)) { atomicMax(error, ERR_STUCK); break; }  // never hang the device on a lost copy
-        }
-        phase ^= 1u << s;
-        pending &= ~(1u << s);
-    }
-};
-
-// ------------------------------------------------------------------------------------------
 // Kernel "scan": the line list is streamed, 32 lines per warp step.
 // ------------------------------------------------------------------------------------------
-template <bool FR, int MIN_CTAS, bool CONT, bool TMA = false>
+template <bool FR, int MIN_CTAS, bool CONT>
 __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
     const KParams &P = cP;
     extern __shared__ double s_bulk[];  // [2 S] per-CTA J and nu_bar rows (this kernel: 3 % faster than the global replicas)
     for (int i = threadIdx.x; i < 2 * P.n_shells; i += blockDim.x) s_bulk[i] = 0.0;
-    TmaRing ring;
-    ring.wb = nullptr; ring.bar = nullptr; ring.phase = 0u; ring.pending = 0u;
-    if (TMA) {
-        double *wb = s_bulk + P.park_off + (size_t)(threadIdx.x >> 5) * tma_doubles_per_warp();  // (16-byte aligned: park_off is even)
-        ring.wb = wb;
-        ring.bar = reinterpret_cast<unsigned long long *>(wb + 4 * TMA_TILE);
-        if ((threadIdx.x & 31) == 0) { mbar_init(ring.bar, 1u); mbar_init(ring.bar + 1, 1u); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     __syncthreads();
     double *s_J = s_bulk, *s_nubar = s_bulk + P.n_shells;
     double *s_ffh = bulk_replica() + 2 * P.n_shells + 4;
@@ -1624,8 +1576,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
     Rng rng;
     rng.start(0u, 0u, 0u);
     rng.ring = threadIdx.x & 31;
-    Lane p;
-    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
+    Lane p = idle_lane();
     bool has = false;
     WarpFeed feed;
     Counters c;
@@ -1640,7 +1591,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
 
         TraceSetup t;
         t.d_boundary = 0.0; t.tau_event = 0.0; t.comov_nu = 0.0; t.chi = 1.0; t.delta_shell = 0;
-        t.chi_bf_tot = 0.0; t.chi_ff = 0.0; t.escat_prob = 1.0; t.dop = 1.0; t.boltz = 0.0; t.cg = -1; t.cn = 0;
+        clear_continuum_fields(t);
         double distance = 0.0, tau_excl_res = 0.0;
         int itype = 0;
         bool need_scan = false;
@@ -1684,28 +1635,14 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
             int res_line = start, res_type = 0;
             double res_excl = 0.0;
             // software prefetch of the first chunk
-            double nu_l, tau_l;
-            int tile = base / TMA_TILE, stage = 0;
-            if (TMA) {
-                // a scan that ended early leaves tiles on their way: let them land before their stages are reused
-                if (ring.pending & 1u) ring.wait(0, P.error);
-                if (ring.pending & 2u) ring.wait(1, P.error);
-                __syncwarp();
-                ring.issue(0, P.nu_line + (size_t)tile * TMA_TILE, tau_row + (size_t)tile * TMA_TILE, lane);
-                if ((tile + 1) * TMA_TILE < P.lpad) ring.issue(1, P.nu_line + (size_t)(tile + 1) * TMA_TILE, tau_row + (size_t)(tile + 1) * TMA_TILE, lane);
-                ring.wait(0, P.error);
-                nu_l = ring.nu(0)[base - tile * TMA_TILE + lane]; tau_l = ring.tau(0)[base - tile * TMA_TILE + lane];
-            } else {
-                nu_l = P.nu_line[base + lane];
-                tau_l = tau_row[base + lane];
-            }
+            double nu_l = P.nu_line[base + lane];
+            double tau_l = tau_row[base + lane];
             while (true) {
                 const int line = base + lane;
                 const bool valid = (line >= start) && (line < L);
                 // prefetch next chunk (speculative; rows are padded so the address is always mapped)
                 const int nbase = (base + 32 < P.lpad) ? base + 32 : base;
-                double nu_next = 0.0, tau_next = 0.0;
-                if (!TMA) { nu_next = P.nu_line[nbase + lane]; tau_next = tau_row[nbase + lane]; }
+                const double nu_next = P.nu_line[nbase + lane], tau_next = tau_row[nbase + lane];
 
                 if (!valid) tau_l = 0.0;
                 double d;
@@ -1753,17 +1690,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
                 carry = shfl_d(incl, 31);
                 base += 32;
                 if (base >= P.lpad) { res_type = IT_BOUNDARY; res_line = L - 1; break; }  // unreachable: line L-1 always breaks
-                if (TMA) {
-                    if (base - tile * TMA_TILE >= TMA_TILE) {  // tile consumed: refill its stage two tiles ahead, move to the other one
-                        __syncwarp();
-                        if ((tile + 2) * TMA_TILE < P.lpad) ring.issue(stage, P.nu_line + (size_t)(tile + 2) * TMA_TILE, tau_row + (size_t)(tile + 2) * TMA_TILE, lane);
-                        tile++; stage ^= 1;
-                        ring.wait(stage, P.error);
-                    }
-                    nu_l = ring.nu(stage)[base - tile * TMA_TILE + lane]; tau_l = ring.tau(stage)[base - tile * TMA_TILE + lane];
-                } else {
-                    nu_l = nu_next; tau_l = tau_next;
-                }
+                nu_l = nu_next; tau_l = tau_next;
             }
             if (lane == j) { p.next_line = res_line; itype = res_type; tau_excl_res = res_excl; }
         }
@@ -1783,10 +1710,6 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
             else interaction_event_impl<FR, CONT>(p, rng, itype, c);  // (on the state itself: see WarpFeed::refill)
             if (p.status != ST_IN_PROCESS) { finish_packet(p, rng, c); has = false; }
         }
-    }
-    if (TMA) {  // no bulk copy may still be writing this CTA's shared memory when it exits
-        if (ring.pending & 1u) ring.wait(0, P.error);
-        if (ring.pending & 2u) ring.wait(1, P.error);
     }
     __syncthreads();
     for (int i = threadIdx.x; i < P.n_shells; i += blockDim.x) {
@@ -1898,6 +1821,43 @@ __device__ __forceinline__ int grid_crossing(const Lane &p, int delta_shell) {
 // state: 0: trace end known (f = g); 1: first true lies in [start, g-1]; 2: search upwards from g; 3: list exhausted
 struct ParkState { TraceSetup t; Brk fb; int g, state; };
 
+// A parked trace in shared memory, one column per field, slot s of `stride` slots (the lane-resident kernel: slot
+// threadIdx.x of blockDim.x; the pooled kernel: a pool slot).  Doubles {d_boundary, tau_event, comov_nu, chi, fb.excl,
+// fb.dcont} (+ continuum mode {chi_bf_tot, chi_ff, escat_prob, dop, boltz}), ints {g, word} (+ continuum mode {cg, cn})
+// with word = state | fb.b << 2 | fb.p1 << 3 | (delta_shell + 1) << 4; bits 9.. of the word belong to the holder.
+__host__ __device__ constexpr int trace_nd(bool cont) { return cont ? 11 : 6; }
+__host__ __device__ constexpr int trace_ni(bool cont) { return cont ? 4 : 2; }
+template <bool CONT>
+struct TraceColumns {
+    double *d; int *i; int stride;
+    __device__ __forceinline__ int &word(int s) const { return i[stride + s]; }
+    __device__ __forceinline__ void put(int s, const ParkState &ps, int high_bits) const {
+        const int n = stride;
+        d[s] = ps.t.d_boundary; d[n + s] = ps.t.tau_event; d[2 * n + s] = ps.t.comov_nu; d[3 * n + s] = ps.t.chi;
+        d[4 * n + s] = ps.fb.excl; d[5 * n + s] = ps.fb.dcont;
+        if (CONT) {
+            d[6 * n + s] = ps.t.chi_bf_tot; d[7 * n + s] = ps.t.chi_ff; d[8 * n + s] = ps.t.escat_prob; d[9 * n + s] = ps.t.dop;
+            d[10 * n + s] = ps.t.boltz; i[2 * n + s] = ps.t.cg; i[3 * n + s] = ps.t.cn;
+        }
+        i[s] = ps.g;
+        word(s) = ps.state | (ps.fb.b ? 4 : 0) | (ps.fb.p1 ? 8 : 0) | ((ps.t.delta_shell + 1) << 4) | high_bits;
+    }
+    __device__ __forceinline__ void get(int s, ParkState &ps) const {
+        const int n = stride;
+        ps.t.d_boundary = d[s]; ps.t.tau_event = d[n + s]; ps.t.comov_nu = d[2 * n + s]; ps.t.chi = d[3 * n + s];
+        ps.fb.excl = d[4 * n + s]; ps.fb.dcont = d[5 * n + s];
+        ps.g = i[s];
+        const int w = word(s);
+        ps.state = w & 3; ps.fb.b = (w & 4) != 0; ps.fb.p1 = (w & 8) != 0; ps.t.delta_shell = ((w >> 4) & 3) - 1;
+        if (CONT) {
+            ps.t.chi_bf_tot = d[6 * n + s]; ps.t.chi_ff = d[7 * n + s]; ps.t.escat_prob = d[8 * n + s]; ps.t.dop = d[9 * n + s];
+            ps.t.boltz = d[10 * n + s]; ps.t.cg = i[2 * n + s]; ps.t.cn = i[3 * n + s];
+        } else {
+            clear_continuum_fields(ps.t);
+        }
+    }
+};
+
 // Phase A of one packet: set the trace up, guess where it ends, verify.  Returns false when the trace ended at the
 // shell boundary (the common case: the packet has been moved and the boundary handled; `has` drops if it left the
 // grid), true when the packet must be parked (ps filled, no side effect on the packet or the estimators yet).
@@ -1907,7 +1867,7 @@ __device__ __forceinline__ bool trace_phase_a(Lane &p, Rng &rng, Counters &c, do
     const KParams &P = cP;
     const int L = P.n_lines;
     TraceSetup &t = ps.t;
-    t.chi_bf_tot = 0.0; t.chi_ff = 0.0; t.escat_prob = 1.0; t.dop = 1.0; t.boltz = 0.0; t.cg = -1; t.cn = 0;
+    clear_continuum_fields(t);
     trace_setup<FR, CONT, true>(p, rng, t);
     const int start = p.next_line;
     ps.g = 0; ps.state = 0;
@@ -1934,29 +1894,7 @@ __device__ __forceinline__ bool trace_phase_a(Lane &p, Rng &rng, Counters &c, do
         } else {
             nu_b = t.comov_nu - t.d_boundary * p.nu * P.inv_ct;
         }
-        int g = L - 1;
-        if (nu_b > 0.0) {
-            // first index with nu_line <= nu_b
-            const long long kb = (__double_as_longlong(nu_b) >> NU_KEY_SHIFT) - P.nu_key_min;
-            if (kb >= (long long)P.n_keys) g = 0;
-            else if (kb >= 0) {
-                int glo = P.nu_first_le[kb];
-                int ghi = (kb > 0) ? P.nu_first_le[kb - 1] : L;
-                if (ghi - glo <= 8) {  // a bucket holds ~2 lines on average: eight independent loads, no dependent chain
-                    // (a lane that needs the bisection below holds up its whole warp: with <= 4 that was 7 % of the traces)
-                    int cnt = 0;  // number of bracket entries that are still > nu_b (the list is sorted; rows are padded)
-#pragma unroll
-                    for (int k = 0; k < 8; k++) cnt += (glo + k < ghi && P.nu_line[glo + k] > nu_b);
-                    g = glo + cnt;
-                } else {
-                    while (glo < ghi) {
-                        const int mid = (glo + ghi) >> 1;
-                        if (P.nu_line[mid] <= nu_b) ghi = mid; else glo = mid + 1;
-                    }
-                    g = glo;
-                }
-            }
-        }
+        int g = first_line_at_or_below(nu_b);
         g = g < start ? start : (g > L - 1 ? L - 1 : g);
         ps.g = g;
         const int gm = (g > start) ? g - 1 : g;
@@ -2040,7 +1978,7 @@ __device__ __forceinline__ bool trace_phase_a(Lane &p, Rng &rng, Counters &c, do
 }
 
 // Phase B of a parked packet: finish the search, apply the estimator range update, move and handle the event.
-template <bool FR, bool CONT, bool DEFER, bool ESC = CONT, bool VP = !CONT>
+template <bool FR, bool CONT, bool DEFER, bool ESC>
 __device__ __forceinline__ void event_phase_b(Lane &p, Rng &rng, Counters &c, double *s_J, double *s_nubar,
                                               double *s_ffh, const TraceSetup &t, Brk fb, int g, int pk_state, bool &has, int &ev_type) {
     const KParams &P = cP;
@@ -2111,24 +2049,22 @@ __device__ __forceinline__ void event_phase_b(Lane &p, Rng &rng, Counters &c, do
         if (ESC) continuum_event_impl(p, rng, t.comov_nu, t.chi_bf_tot, t.chi_ff, c);
         else continuum_event(p, rng, t.comov_nu, t.chi_bf_tot, t.chi_ff, c);
     }
-    else if (ESC) interaction_event_impl<FR, CONT, VP>(p, rng, itype, c);
-    else interaction_event<FR, CONT, VP>(p, rng, itype, c);
+    else if (ESC) interaction_event_impl<FR, CONT, false>(p, rng, itype, c);
+    else interaction_event<FR, CONT, false>(p, rng, itype, c);
     if (p.status != ST_IN_PROCESS) { if (!DEFER) finish_packet(p, rng, c); has = false; }
 }
 
-// Kernel "jump", lane-resident form (used for the continuum mode): one packet per lane; a parked packet keeps its
-// lane idle until park_min lanes of the warp wait (its trace state waits in a per-thread shared-memory column).
-// WVOL (classic mode with virtual packets): the volleys run warp-cooperatively (warp_volley) instead of per lane.
-template <bool FR, int MIN_CTAS, bool CONT, bool ESC = CONT, bool WVOL = false>
+// Kernel "jump", lane-resident form (when the pools do not fit or with option pooled = 0; classic mode with virtual
+// packets): one packet per lane; a parked packet keeps its lane idle until park_min lanes of the warp wait (its trace state waits
+// in a per-thread shared-memory column).
+// WVOL (classic mode with virtual packets): the volleys run warp-cooperatively (warp_volley).
+template <bool FR, int MIN_CTAS, bool CONT, bool WVOL = false>
 __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
+    // ESC: the rare handlers work on the packet state itself (see WarpFeed::refill and event_phase_b)
+    constexpr bool ESC = CONT || WVOL;
     const KParams &P = cP;
     extern __shared__ double s_bulk[];  // jump kernels: [4 S] shell table, then the parked-lane columns
-    // [4 S] shell table {r_inner, r_outer, chi_e, 1 / chi_e} (+ [S + 5 n_continua S] continuum estimators when they fit)
-    for (int i = threadIdx.x; i < P.n_shells; i += blockDim.x) {
-        const double chi_e = P.n_e[i] * P.sigma_thomson;
-        s_bulk[i] = P.r_inner[i]; s_bulk[P.n_shells + i] = P.r_outer[i];
-        s_bulk[2 * P.n_shells + i] = chi_e; s_bulk[3 * P.n_shells + i] = 1.0 / chi_e;
-    }
+    load_shell_table();
     __syncthreads();
     double *s_J = bulk_replica(), *s_nubar = s_J + P.n_shells;
     double *s_ffh = s_J + 2 * P.n_shells + 4;
@@ -2136,23 +2072,20 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
     Rng rng;
     rng.start(0u, 0u, 0u);
     rng.ring = threadIdx.x & 31;
-    Lane p;
-    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
+    Lane p = idle_lane();
     bool has = false, parked = false, vpend = false;
     WarpFeed feed;
     Counters c;
     // The state of a PARKED lane (its trace set-up and what the guess already established) waits in shared memory,
-    // one column per thread, not in ~20 registers carried through phase A: [NPD doubles][3 (classic) or 5 (continuum) ints] x blockDim.x.
-    constexpr int NPD = CONT ? 11 : 6;
-    double *pk_d = s_bulk + P.park_off + threadIdx.x;
-    int *pk_i = reinterpret_cast<int *>(s_bulk + P.park_off + NPD * blockDim.x) + threadIdx.x;
-    const int BD = blockDim.x;
+    // one column per thread, not in ~20 registers carried through phase A.
+    const TraceColumns<CONT> park{s_bulk + P.park_off, reinterpret_cast<int *>(s_bulk + P.park_off + trace_nd(CONT) * blockDim.x),
+                                  (int)blockDim.x};
 
     bool done = false;  // holds a packet that has left the grid; finish_packet runs batched, inside refill
     unsigned pass = 0;
     while (true) {
         const bool had_before = has;
-        feed.refill<FR, ESC, !CONT && !WVOL>(p, rng, has, __ballot_sync(FULL, has), c, done);
+        feed.refill<FR, ESC, false>(p, rng, has, __ballot_sync(FULL, has), c, done);
         if (__ballot_sync(FULL, has || done) == 0u) break;
         if (WVOL) {
             // A packet that owes a volley (at birth, packet_propagation.py:109-118; after a line interaction or an electron
@@ -2174,12 +2107,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
         if (has && !parked && !(WVOL && vpend)) {
             ParkState ps;
             if (trace_phase_a<FR, CONT, true>(p, rng, c, s_J, s_nubar, s_ffh, ps, has)) {
-                const TraceSetup &t = ps.t;
-                pk_d[0] = t.d_boundary; pk_d[BD] = t.tau_event; pk_d[2 * BD] = t.comov_nu; pk_d[3 * BD] = t.chi;
-                pk_d[4 * BD] = ps.fb.excl; pk_d[5 * BD] = ps.fb.dcont;
-                if (CONT) { pk_d[6 * BD] = t.chi_bf_tot; pk_d[7 * BD] = t.chi_ff; pk_d[8 * BD] = t.escat_prob; pk_d[9 * BD] = t.dop; pk_d[10 * BD] = t.boltz; }
-                pk_i[0] = ps.g; pk_i[BD] = t.delta_shell; pk_i[2 * BD] = ps.state | (ps.fb.b ? 4 : 0) | (ps.fb.p1 ? 8 : 0);
-                if (CONT) { pk_i[3 * BD] = t.cg; pk_i[4 * BD] = t.cn; }
+                park.put(threadIdx.x, ps, 0);
                 parked = true;
             }
         }
@@ -2190,19 +2118,10 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
         if (parked_mask != 0u && (__popc(parked_mask) >= P.park_min || runnable == 0u)) {
             int ev_type = IT_BOUNDARY;
             if (parked) {
-                TraceSetup t;
-                t.d_boundary = pk_d[0]; t.tau_event = pk_d[BD]; t.comov_nu = pk_d[2 * BD]; t.chi = pk_d[3 * BD];
-                Brk fb;
-                fb.excl = pk_d[4 * BD]; fb.dcont = pk_d[5 * BD];
-                if (CONT) { t.chi_bf_tot = pk_d[6 * BD]; t.chi_ff = pk_d[7 * BD]; t.escat_prob = pk_d[8 * BD]; t.dop = pk_d[9 * BD]; t.boltz = pk_d[10 * BD];
-                            t.cg = pk_i[3 * BD]; t.cn = pk_i[4 * BD]; }
-                else { t.chi_bf_tot = 0.0; t.chi_ff = 0.0; t.escat_prob = 1.0; t.dop = 1.0; t.boltz = 0.0; t.cg = -1; t.cn = 0; }
-                const int g = pk_i[0];
-                t.delta_shell = pk_i[BD];
-                const int flags = pk_i[2 * BD];
-                fb.b = (flags & 4) != 0; fb.p1 = (flags & 8) != 0;
+                ParkState ps;
+                park.get(threadIdx.x, ps);
                 // (inline on purpose: an out-of-line phase B with copied packet state measured 15 % slower)
-                event_phase_b<FR, CONT, true, ESC, !CONT && !WVOL>(p, rng, c, s_J, s_nubar, s_ffh, t, fb, g, flags & 3, has, ev_type);
+                event_phase_b<FR, CONT, true, ESC>(p, rng, c, s_J, s_nubar, s_ffh, ps.t, ps.fb, ps.g, ps.state, has, ev_type);
                 parked = false;
             }
             if (WVOL && ev_type != IT_BOUNDARY && has) vpend = true;  // owes a volley now (see above)
@@ -2220,53 +2139,36 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_jump_kernel() {
 // park_min packets are parked the lanes swap their runnable packets against parked ones (which stashes the runnable
 // ones in the very same slots), handle the events, and carry on tracing with the packets they just handled.
 // A packet's trajectory does not depend on where it waits: its RNG state, ring id and seg_open bit travel with it.
-// Pool slot = [POOL_ND doubles][POOL_NI ints], slot index fastest (conflict-free: lanes use distinct slots).
+// Pool slot = [POOL_ND doubles][POOL_NI ints], slot index fastest (conflict-free: lanes use distinct slots): the packet's
+// 4 doubles, then its parked trace's doubles; the packet's ints {pid, next_line, shell, icount, bbuf, nev, nsteps, rng n,
+// a, b}, the parked trace's ints (TraceColumns, whose word holds the slot's ring id in bits 9..), then seg_open.
 // ------------------------------------------------------------------------------------------
-// (continuum mode: five more doubles {chi_bf_tot, chi_ff, escat_prob, dop, boltz} and two more ints {bin, active continua})
-__host__ __device__ constexpr int pool_nd(bool cont) { return cont ? 15 : 10; }
-__host__ __device__ constexpr int pool_ni(bool cont) { return cont ? 15 : 13; }
+__host__ __device__ constexpr int pool_nd(bool cont) { return 4 + trace_nd(cont); }
+__host__ __device__ constexpr int pool_ni(bool cont) { return 10 + trace_ni(cont) + 1; }
 __host__ __device__ constexpr int pool_bytes_per_slot(bool cont) { return pool_nd(cont) * 8 + pool_ni(cont) * 4 + 4; }  // + one int of the per-warp slot list
 
 template <bool CONT>
 struct PoolView {
     double *d; int *i; int *list; int ns;
-    // packet part of a slot (the ring id lives in bits 9.. of the packed word and always travels with the context)
+    // the slot's parked trace (derived where it is used: the pooled kernels sit at their register limit)
+    __device__ __forceinline__ TraceColumns<CONT> trace() const { return TraceColumns<CONT>{d + 4 * ns, i + 10 * ns, ns}; }
+    // packet part of a slot (the ring id lives in bits 9.. of the trace word and always travels with the context)
     __device__ __forceinline__ void put_packet(int s, const Lane &q, const Rng &r) const {
         d[s] = q.r; d[ns + s] = q.mu; d[2 * ns + s] = q.nu; d[3 * ns + s] = q.energy;
         i[s] = q.pid; i[ns + s] = q.next_line; i[2 * ns + s] = q.shell; i[3 * ns + s] = q.icount; i[4 * ns + s] = q.bbuf;
         i[5 * ns + s] = q.nev; i[6 * ns + s] = q.nsteps; i[7 * ns + s] = (int)r.n; i[8 * ns + s] = (int)r.a; i[9 * ns + s] = (int)r.b;
-        i[12 * ns + s] = q.seg_open;
+        i[(10 + trace_ni(CONT)) * ns + s] = q.seg_open;
     }
     __device__ __forceinline__ void get_packet(int s, Lane &q, Rng &r) const {
         q.r = d[s]; q.mu = d[ns + s]; q.nu = d[2 * ns + s]; q.energy = d[3 * ns + s];
         q.pid = i[s]; q.next_line = i[ns + s]; q.shell = i[2 * ns + s]; q.icount = i[3 * ns + s]; q.bbuf = i[4 * ns + s];
         q.nev = i[5 * ns + s]; q.nsteps = i[6 * ns + s]; r.n = (unsigned)i[7 * ns + s]; r.a = (unsigned)i[8 * ns + s]; r.b = (unsigned)i[9 * ns + s];
-        q.seg_open = i[12 * ns + s];
+        q.seg_open = i[(10 + trace_ni(CONT)) * ns + s];
         q.status = ST_IN_PROCESS; r.pid = (unsigned)q.pid;
     }
-    __device__ __forceinline__ void put_trace(int s, const ParkState &ps, unsigned ring) const {
-        d[4 * ns + s] = ps.t.d_boundary; d[5 * ns + s] = ps.t.tau_event; d[6 * ns + s] = ps.t.comov_nu; d[7 * ns + s] = ps.t.chi;
-        d[8 * ns + s] = ps.fb.excl; d[9 * ns + s] = ps.fb.dcont;
-        if (CONT) {
-            d[10 * ns + s] = ps.t.chi_bf_tot; d[11 * ns + s] = ps.t.chi_ff; d[12 * ns + s] = ps.t.escat_prob; d[13 * ns + s] = ps.t.dop;
-            d[14 * ns + s] = ps.t.boltz; i[13 * ns + s] = ps.t.cg; i[14 * ns + s] = ps.t.cn;
-        }
-        i[10 * ns + s] = ps.g;
-        i[11 * ns + s] = ps.state | (ps.fb.b ? 4 : 0) | (ps.fb.p1 ? 8 : 0) | ((ps.t.delta_shell + 1) << 4) | (int)(ring << 9);
-    }
-    __device__ __forceinline__ void put_ring(int s, unsigned ring) const { i[11 * ns + s] = (int)(ring << 9); }
-    __device__ __forceinline__ unsigned get_ring(int s) const { return (unsigned)i[11 * ns + s] >> 9; }
-    __device__ __forceinline__ void get_trace(int s, TraceSetup &t, Brk &fb, int &g, int &state) const {
-        t.d_boundary = d[4 * ns + s]; t.tau_event = d[5 * ns + s]; t.comov_nu = d[6 * ns + s]; t.chi = d[7 * ns + s];
-        fb.excl = d[8 * ns + s]; fb.dcont = d[9 * ns + s];
-        g = i[10 * ns + s];
-        const int w = i[11 * ns + s];
-        state = w & 3; fb.b = (w & 4) != 0; fb.p1 = (w & 8) != 0; t.delta_shell = ((w >> 4) & 3) - 1;
-        if (CONT) {
-            t.chi_bf_tot = d[10 * ns + s]; t.chi_ff = d[11 * ns + s]; t.escat_prob = d[12 * ns + s]; t.dop = d[13 * ns + s];
-            t.boltz = d[14 * ns + s]; t.cg = i[13 * ns + s]; t.cn = i[14 * ns + s];
-        } else { t.chi_bf_tot = 0.0; t.chi_ff = 0.0; t.escat_prob = 1.0; t.dop = 1.0; t.boltz = 0.0; t.cg = -1; t.cn = 0; }
-    }
+    __device__ __forceinline__ void put_trace(int s, const ParkState &ps, unsigned ring) const { trace().put(s, ps, (int)(ring << 9)); }
+    __device__ __forceinline__ void put_ring(int s, unsigned ring) const { trace().word(s) = (int)(ring << 9); }
+    __device__ __forceinline__ unsigned get_ring(int s) const { return (unsigned)trace().word(s) >> 9; }
     // list[k] = index of the k-th set bit of `first`, then of `second` (both uniform across the warp)
     __device__ __forceinline__ void rank_slots(unsigned long long first, unsigned long long second, int lane) const {
         const int nfirst = __popcll(first);
@@ -2292,11 +2194,7 @@ template <bool FR, int MIN_CTAS, bool CONT = false>
 __global__ void __launch_bounds__(256, MIN_CTAS) transport_pool_kernel() {
     const KParams &P = cP;
     extern __shared__ double s_bulk[];  // [4 S] shell table, then the per-warp pools
-    for (int i = threadIdx.x; i < P.n_shells; i += blockDim.x) {  // shell table, see trace_setup
-        const double chi_e = P.n_e[i] * P.sigma_thomson;
-        s_bulk[i] = P.r_inner[i]; s_bulk[P.n_shells + i] = P.r_outer[i];
-        s_bulk[2 * P.n_shells + i] = chi_e; s_bulk[3 * P.n_shells + i] = 1.0 / chi_e;
-    }
+    load_shell_table();
     double *s_J = bulk_replica(), *s_nubar = s_J + P.n_shells;
     double *s_ffh = s_J + 2 * P.n_shells + 4;
 
@@ -2319,8 +2217,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_pool_kernel() {
     Rng rng;
     rng.start(0u, 0u, 0u);
     rng.ring = (unsigned)lane;
-    Lane p;
-    p.status = -1; p.pid = -1; p.r = p.mu = p.nu = p.energy = 0.0; p.next_line = 0; p.shell = 0; p.icount = 0; p.bbuf = 0; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
+    Lane p = idle_lane();
     bool has = false;
     WarpFeed feed;
     Counters c;
@@ -2404,15 +2301,15 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_pool_kernel() {
             int s = 0;
             if (take) {
                 s = pool.list[lane];
-                Lane q; Rng qr; TraceSetup t; Brk fb; int g, state;
+                Lane q; Rng qr; ParkState pk;
                 qr.ring = pool.get_ring(s);
                 pool.get_packet(s, q, qr);
-                pool.get_trace(s, t, fb, g, state);
+                pool.trace().get(s, pk);
                 if (had) { pool.put_packet(s, p, rng); pool.put_ring(s, rng.ring); }  // stash the runnable packet this lane held
                 else pool.put_ring(s, rng.ring);
                 p = q; rng = qr; has = true;
                 int ev_type;
-                event_phase_b<FR, CONT, false, false, false>(p, rng, c, s_J, s_nubar, s_ffh, t, fb, g, state, has, ev_type);
+                event_phase_b<FR, CONT, false, false>(p, rng, c, s_J, s_nubar, s_ffh, pk.t, pk.fb, pk.g, pk.state, has, ev_type);
             }
             const unsigned long long used = warp_or_slot(take, s);
             parked &= ~used;
@@ -2531,11 +2428,10 @@ __global__ void order_scan_kernel(unsigned *hist, int n_keys) {
         __syncthreads();
     }
 }
-__global__ void order_scatter_kernel(const double *nu, long long n, int shift, long long key_min, int n_keys, unsigned *cursor, int *order, int use_local) {
+__global__ void order_scatter_kernel(const double *nu, long long n, int shift, long long key_min, int n_keys, unsigned *cursor, int *order) {
     __shared__ unsigned sh[ORDER_SMEM_KEYS];  // count of the block per key, then the block's first slot of the key
-    const bool local = use_local && n_keys <= ORDER_SMEM_KEYS;
     const long long base = (long long)blockIdx.x * blockDim.x * ORDER_ITEMS;
-    if (!local) {
+    if (n_keys > ORDER_SMEM_KEYS) {  // too many keys for the block's counters: one global atomic per packet
         for (int q = 0; q < ORDER_ITEMS; q++) {
             const long long i = base + (long long)q * blockDim.x + threadIdx.x;
             if (i < n) order[atomicAdd(&cursor[order_key(nu[i], shift, key_min, n_keys)], 1u)] = (int)i;

@@ -92,9 +92,10 @@ class Engine:
 
     def set_option(self, name: str, value: int):
         """Tuning knobs of `tb200_set_option`; none of them changes a result.  algorithm (1 jump, 0 scan), pooled (1),
-        ctas_per_sm / park_min (0 = measured best for the kernel that will run), threads_per_cta (256 | 128),
+        ctas_per_sm / park_min (0 = measured best for the kernel that will run; each kernel is compiled for its default CTAs
+        per SM, so another ctas_per_sm only sizes the grid, at most to what fits), threads_per_cta (256 | 128), vol_min (24),
         refill_min (0 = 12 pooled classic / 8 otherwise), sort_packets (1), sort_bits (5), pipeline_chunks (8), pipeline_edges (1: the first and last
-        packet range of `run` are a quarter of the others)."""
+        packet range of `run` are a quarter of the others), keep_opacity_tables (0).  An unknown name raises."""
         self._check(self._lib.tb200_set_option(self._h, name.encode(), int(value)))
 
     # ---- tables ----

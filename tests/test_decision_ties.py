@@ -204,7 +204,6 @@ POOLED = {"algorithm": 1, "pooled": 1}
 LANE = {"algorithm": 1, "pooled": 0}
 VOLLEY_1 = {"algorithm": 1, "vol_min": 1}
 VOLLEY_32 = {"algorithm": 1, "vol_min": 32}
-LANE_VOLLEYS = {"algorithm": 1, "warp_volley": 0, "ctas_per_sm": 4}  # transport_jump_kernel<FR, 4, false, true>
 
 
 def check_kernel(options, cases):
@@ -434,7 +433,7 @@ def vpacket_tie_cases(full_rel):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kernel", [VOLLEY_1, VOLLEY_32, LANE_VOLLEYS, SCAN], ids=["volley_min1", "volley_min32", "lane_volleys", "scan"])
+@pytest.mark.parametrize("kernel", [VOLLEY_1, VOLLEY_32, SCAN], ids=["volley_min1", "volley_min32", "scan"])
 @pytest.mark.parametrize("full_rel", [False, True], ids=["partial_rel", "full_rel"])
 def test_vpacket_window_ties_match_the_oracle(kernel, full_rel):
     check_kernel(kernel, vpacket_tie_cases(full_rel))
@@ -559,7 +558,7 @@ def clustered_cases(vpackets: int):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kernel,vpackets", [(SCAN, 0), (POOLED, 0), (LANE, 0), (VOLLEY_1, 3), (LANE_VOLLEYS, 3), (SCAN, 3)],
-                         ids=["scan", "pooled", "lane", "volley", "lane_volleys", "scan_vpackets"])
+@pytest.mark.parametrize("kernel,vpackets", [(SCAN, 0), (POOLED, 0), (LANE, 0), (VOLLEY_1, 3), (SCAN, 3)],
+                         ids=["scan", "pooled", "lane", "volley", "scan_vpackets"])
 def test_clustered_line_list_matches_the_oracle(kernel, vpackets):
     check_kernel(kernel, clustered_cases(vpackets))

@@ -458,21 +458,6 @@ def test_pooled_kernel_scheduling_is_invisible(oracle, park_min, refill_min, cta
         assert_close(res[k], ref[k], 1e-10, k)
 
 
-@pytest.mark.parametrize("name", ["scatter_basic", "macroatom_basic", "scatter_thick"])
-def test_scan_kernel_with_tma_staging_matches_golden(name):
-    """Engine option scan_tma: the streaming kernel reads its line-list tiles through cp.async.bulk + mbarrier."""
-    from tardis_b200.engine import Engine
-
-    model, packets, rk, sig, g = load_case(name)
-    eng = Engine(0)
-    eng.set_option("algorithm", 0)
-    eng.set_option("scan_tma", 1)
-    eng.set_model_from(model, **engine_config(rk, sig))
-    res = eng.run_packets(packets, track_last_interaction=True, n_tracked_packets=make_golden.N_TRACKED, max_events_per_packet=4096)
-    compare_to_golden(res, g, make_golden.N_TRACKED)
-    eng.close()
-
-
 @pytest.mark.parametrize("vol_min", [1, 32])
 def test_warp_volley_batching_does_not_change_results(oracle, vol_min):
     """The warp-cooperative volleys give the oracle's numbers whether they run for one waiting packet or for a full warp."""
