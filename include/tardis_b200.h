@@ -18,9 +18,11 @@
  * the call that receives them.  Device memory is library-owned and persists
  * across MC iterations.  Every function returns TB200_OK (0) or an error code;
  * tb200_last_error() gives the message.  One engine drives one GPU from one
- * host thread; multi-GPU = one process (and engine) per GPU, packets sharded
- * by the caller, estimators summed across ranks through the device buffer
- * exposed by tb200_estimator_buffer() (see INTEGRATION.md).
+ * host thread.  Multi-GPU from one process: an engine group (tb200_group_*,
+ * end of this file) drives one engine per listed device and sums their
+ * estimators itself.  Across processes or nodes: one engine per rank, packets
+ * sharded by the caller, estimators summed through the device buffer exposed
+ * by tb200_estimator_buffer() (see INTEGRATION.md).
  */
 #ifndef TARDIS_B200_H
 #define TARDIS_B200_H
@@ -354,6 +356,52 @@ int64_t tb200_kernel_launches(tb200_engine *engine);                 /* kernels 
  * packet range of tb200_run are a quarter of the others, their copies being the ones no kernel hides), "keep_opacity_tables".
  * Any other name is an error. */
 int tb200_set_option(tb200_engine *engine, const char *name, int64_t value);
+
+/* ---- engine groups: one MC iteration on several GPUs from one host call ----
+ * A group owns one ordinary engine per entry of device_ids; an id may repeat ({0, 0} is two engines on device 0).
+ * tb200_group_member exposes the members, so every single-engine call stays usable on one.  The tb200_group_* calls
+ * below apply to every member, one host thread per member; an error names the member (and, for runs, its global packet
+ * range: the kernels record an error code, not the index of the packet that raised it) and leaves the group usable.
+ * Members on the same device transport one after the other.
+ *
+ * tb200_group_run: member g transports packets [g N / G, (g + 1) N / G) of the caller's arrays (no host copies) at the
+ * fixed-point scales of the whole set, and writes its per-packet outputs and last-interaction columns straight into the
+ * caller's arrays at that offset.  TrackerFull rows cover global packets [0, n_tracked_packets) with global packet_id;
+ * the virtual-packet log is concatenated in member order with global vlog_packet_index, vlog_count is the total (rows
+ * beyond vlog_capacity are dropped, as with one engine; every member keeps a device log of vlog_capacity rows, and only the
+ * rows that fit are copied to the caller).  Then tb200_group_allreduce, and the estimators come back as
+ * from one engine: J_blue / Edotlu and the counters bit-identical to one engine over the same packets, the other sums
+ * to rounding.
+ * tb200_group_create_packets: member g generates exactly packets [g N / G, (g + 1) N / G) of what tb200_create_packets
+ * gives one engine, in place (the set never passes through one device).  tb200_group_run_resident then runs them.
+ * tb200_group_allreduce: the collective alone (for callers that drive tb200_transport per member), once per transport: a
+ * second call without a transport in between fails (it would add the sums again).  Every member ends up with the same
+ * estimator buffer.  *exact = 1: every member ran the jump algorithm at the same fixed-point scales, so
+ * the line accumulators were summed as integers and finalized, and [0, off_j_blue) of the estimator buffer was summed
+ * in f64 in member order; *exact = 0: the whole buffer was summed in f64 in member order.  Members whose devices have
+ * peer access read each other's memory; the others (and all, with the option "peer_access" = 0) are staged through
+ * cudaMemcpyPeerAsync.
+ * tb200_group_formal_integral: member g integrates frequencies [g n / G, (g + 1) n / G); every member needs the
+ * source-function tables (tb200_solve_source_function on each member: identical inputs give identical tables). */
+typedef struct tb200_group tb200_group;
+int tb200_group_create(const int *device_ids, int n, tb200_group **group);
+void tb200_group_destroy(tb200_group *group);
+int tb200_group_size(tb200_group *group);
+int tb200_group_member(tb200_group *group, int i, tb200_engine **engine);
+int tb200_group_set_option(tb200_group *group, const char *name, int64_t value); /* "peer_access" (1), or any engine option */
+int tb200_group_set_model(tb200_group *group, const tb200_model *model, const tb200_config *config);
+int tb200_group_set_atomic_data(tb200_group *group, const tb200_atomic_data *atomic);
+int tb200_group_build_opacity(tb200_group *group, const tb200_plasma_state *plasma);
+int tb200_group_upload_packets(tb200_group *group, const tb200_packets *packets);
+int tb200_group_create_packets(tb200_group *group, const tb200_packet_source *source);
+int tb200_group_run(tb200_group *group, const tb200_packets *packets, tb200_outputs *outputs);
+int tb200_group_run_resident(tb200_group *group, tb200_outputs *outputs);
+int tb200_group_sync(tb200_group *group);
+int tb200_group_allreduce(tb200_group *group, int *exact);
+int tb200_group_allreduce_ms(tb200_group *group, double *ms); /* host time of the last collective, device work included */
+int tb200_group_formal_integral(tb200_group *group, const tb200_formal_integral_params *params, const double *frequencies,
+                                int64_t n_frequencies, double *luminosity_densities, double *intensities_nu_p);
+int tb200_group_formal_integral_ms(tb200_group *group, double *interpolation_ms, double *integral_ms); /* slowest member's */
 
 #ifdef __cplusplus
 }

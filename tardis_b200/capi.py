@@ -17,6 +17,10 @@ EXPORTED_SYMBOLS = [
     "tb200_set_atomic_data", "tb200_build_opacity", "tb200_download_opacity",
     "tb200_line_accumulators", "tb200_finalize_line_estimators", "tb200_run_resident", "tb200_solve_source_function",
     "tb200_formal_integral", "tb200_formal_integral_ms",
+    "tb200_group_create", "tb200_group_destroy", "tb200_group_size", "tb200_group_member", "tb200_group_set_option",
+    "tb200_group_set_model", "tb200_group_set_atomic_data", "tb200_group_build_opacity", "tb200_group_upload_packets",
+    "tb200_group_create_packets", "tb200_group_run", "tb200_group_run_resident", "tb200_group_sync", "tb200_group_allreduce",
+    "tb200_group_allreduce_ms", "tb200_group_formal_integral", "tb200_group_formal_integral_ms",
 ]
 
 
@@ -207,12 +211,31 @@ def load(build_if_missing: bool = True):
     lib.tb200_solve_source_function.argtypes = [E, C.POINTER(SourceFunctionParams), _pd, _pd, _pd, _pd, C.POINTER(C.c_int32)]
     lib.tb200_formal_integral.argtypes = [E, C.POINTER(FormalIntegralParams), _pd, C.c_int64, _pd, _pd]
     lib.tb200_formal_integral_ms.argtypes = [E, _pd, _pd]
+    lib.tb200_group_create.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(E)]
+    lib.tb200_group_destroy.argtypes = [E]
+    lib.tb200_group_destroy.restype = None
+    lib.tb200_group_size.argtypes = [E]
+    lib.tb200_group_member.argtypes = [E, C.c_int, C.POINTER(E)]
+    lib.tb200_group_set_option.argtypes = [E, C.c_char_p, C.c_int64]
+    lib.tb200_group_set_model.argtypes = [E, C.POINTER(Model), C.POINTER(Config)]
+    lib.tb200_group_set_atomic_data.argtypes = [E, C.POINTER(AtomicData)]
+    lib.tb200_group_build_opacity.argtypes = [E, C.POINTER(PlasmaState)]
+    lib.tb200_group_upload_packets.argtypes = [E, C.POINTER(Packets)]
+    lib.tb200_group_create_packets.argtypes = [E, C.POINTER(PacketSource)]
+    lib.tb200_group_run.argtypes = [E, C.POINTER(Packets), C.POINTER(Outputs)]
+    lib.tb200_group_run_resident.argtypes = [E, C.POINTER(Outputs)]
+    lib.tb200_group_sync.argtypes = [E]
+    lib.tb200_group_allreduce.argtypes = [E, C.POINTER(C.c_int)]
+    lib.tb200_group_allreduce_ms.argtypes = [E, _pd]
+    lib.tb200_group_formal_integral.argtypes = [E, C.POINTER(FormalIntegralParams), _pd, C.c_int64, _pd, _pd]
+    lib.tb200_group_formal_integral_ms.argtypes = [E, _pd, _pd]
     for name in ("tb200_create", "tb200_set_model", "tb200_run", "tb200_upload_packets", "tb200_transport", "tb200_sync",
                  "tb200_download", "tb200_estimator_buffer", "tb200_last_kernel_ms", "tb200_get_counters", "tb200_set_option",
                  "tb200_create_packets", "tb200_download_packets", "tb200_get_estimator_layout", "tb200_solve_radiation_field",
                  "tb200_set_atomic_data", "tb200_build_opacity", "tb200_download_opacity", "tb200_line_accumulators",
                  "tb200_finalize_line_estimators", "tb200_run_resident",
-                 "tb200_solve_source_function", "tb200_formal_integral", "tb200_formal_integral_ms"):
+                 "tb200_solve_source_function", "tb200_formal_integral", "tb200_formal_integral_ms",
+                 *(n for n in EXPORTED_SYMBOLS if n.startswith("tb200_group_") and n != "tb200_group_destroy")):
         getattr(lib, name).restype = C.c_int
     _lib = lib
     return lib

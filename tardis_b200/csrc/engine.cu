@@ -95,8 +95,10 @@ struct tb200_engine {
     DBuf<unsigned long long> diff;  // jump algorithm: [S][lpad+1][4] fixed-point difference arrays
     DBuf<unsigned long long> xfer;  // jump algorithm: [S-1][lpad+1][4] shell-crossing transfers, folded into diff per call
     double e_typ = 0.0;             // typical packet energy (sets the fixed-point scale)
+    double e_typ_group = 0.0;       // > 0: imposed by an engine group for the call in progress (the whole set's e_typ)
     double diff_scale1 = 0.0, diff_scale2 = 0.0;  // scales of what the difference arrays hold (0 = they are empty)
     double finalize_ms = 0.0;
+    bool est_unreduced = false;     // a transport filled the estimators since the last engine-group collective
     DBuf<int> line2macro, block_edge, ttype, dest, tline;
     // continuum (IIP mode)
     int continuum = 0, n_continua = 0, n_phot = 0, phot_pad = 0, n_activation = 0, n_markov = 0;
@@ -518,6 +520,19 @@ static int prepare_tracking(tb200_engine *en, const tb200_outputs *o) {
     return TB200_OK;
 }
 
+// Typical packet energy: mean |energy| over a strided sample of at most 65536 packets.
+static double typical_energy(const double *energies, int64_t n) {
+    const int64_t m = n < 65536 ? n : 65536;
+    double acc = 0.0;
+    for (int64_t i = 0; i < m; i++) acc += fabs(energies[i * (n / m)]);
+    return acc / (double)m;
+}
+
+static void set_typical_energy(tb200_engine *en, const tb200_packets *pk) {
+    if (en->e_typ_group > 0) en->e_typ = en->e_typ_group;
+    else if (pk->n_packets > 0) en->e_typ = typical_energy(pk->initial_energies, pk->n_packets);
+}
+
 int tb200_upload_packets(tb200_engine *en, const tb200_packets *pk) {
     if (!en || !pk) return fail(TB200_ERR_INVALID, "bad argument");
     if (pk->n_packets < 0 || pk->n_packets > 2000000000LL) return fail(TB200_ERR_INVALID, "n_packets out of range");
@@ -529,13 +544,8 @@ int tb200_upload_packets(tb200_engine *en, const tb200_packets *pk) {
         (r = en->out_nu.ensure(n)) || (r = en->out_energy.ensure(n)) || (r = en->seeds64.ensure(n)) || (r = en->seed32.ensure(n)) ||
         (r = en->x397.ensure(n)))
         return r;
+    set_typical_energy(en, pk);
     if (n == 0) return TB200_OK;
-    {
-        const int64_t m = n < 65536 ? n : 65536;
-        double acc = 0.0;
-        for (int64_t i = 0; i < m; i++) acc += fabs(pk->initial_energies[i * (n / m)]);
-        en->e_typ = acc / (double)m;
-    }
     CK(cudaMemcpyAsync(en->in_r.p, pk->initial_radii, n * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->in_nu.p, pk->initial_nus, n * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->in_mu.p, pk->initial_mus, n * sizeof(double), cudaMemcpyHostToDevice, en->stream));
@@ -566,27 +576,31 @@ __global__ void packet_source_scan_kernel(tbps::Pcg64 origin, unsigned long long
     }
 }
 
-__global__ void packet_source_fill_kernel(tbps::SourceParams P, double *r, double *nu, double *mu, double *e, long long *seeds) {
+// Packets [lo, hi) of the P.n the source creates; the arrays hold that range only (element i - lo is packet i).
+__global__ void packet_source_fill_kernel(tbps::SourceParams P, unsigned long long lo, unsigned long long hi, double *r, double *nu,
+                                          double *mu, double *e, long long *seeds) {
     const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned long long i0 = t * PS_CHUNK;
-    if (i0 >= P.n) return;
-    const unsigned long long i1 = (i0 + PS_CHUNK < P.n) ? i0 + PS_CHUNK : P.n;
-    tbps::fill_chunk(P, i0, i1, r, nu, mu, e, seeds);
+    const unsigned long long i0 = lo + t * PS_CHUNK;
+    if (i0 >= hi) return;
+    const unsigned long long i1 = (i0 + PS_CHUNK < hi) ? i0 + PS_CHUNK : hi;
+    tbps::fill_chunk(P, i0, i1, r, nu, mu, e, seeds, lo);
 }
 }  // namespace
 
-int tb200_create_packets(tb200_engine *en, const tb200_packet_source *src) {
+// Packets [lo, hi) of the source's n_packets become the engine's resident packets 0 .. hi - lo - 1, bit for bit what
+// the whole set holds there (an engine group generates each member's range in place).
+static int create_packets_range(tb200_engine *en, const tb200_packet_source *src, int64_t lo, int64_t hi) {
     if (!en || !src) return fail(TB200_ERR_INVALID, "bad argument");
     if (src->n_packets < 0 || src->n_packets > 2000000000LL) return fail(TB200_ERR_INVALID, "n_packets out of range");
     if (!src->l_array || src->n_l < 1 || src->n_l > (1 << 24)) return fail(TB200_ERR_INVALID, "l_array missing");
     if (!(src->temperature > 0) || !(src->radius > 0)) return fail(TB200_ERR_INVALID, "temperature and radius must be positive");
     CK(cudaSetDevice(en->device));
-    const int64_t n = src->n_packets;
-    en->N = n;
+    const int64_t n = src->n_packets, count = hi - lo;
+    en->N = count;
     int r;
-    if ((r = en->in_r.ensure(n)) || (r = en->in_nu.ensure(n)) || (r = en->in_mu.ensure(n)) || (r = en->in_energy.ensure(n)) ||
-        (r = en->out_nu.ensure(n)) || (r = en->out_energy.ensure(n)) || (r = en->seeds64.ensure(n)) || (r = en->seed32.ensure(n)) ||
-        (r = en->x397.ensure(n)) || (r = en->ps_l_array.ensure((size_t)src->n_l)) || (r = en->ps_rejected.ensure(PS_MAX_REJECTED)) ||
+    if ((r = en->in_r.ensure(count)) || (r = en->in_nu.ensure(count)) || (r = en->in_mu.ensure(count)) || (r = en->in_energy.ensure(count)) ||
+        (r = en->out_nu.ensure(count)) || (r = en->out_energy.ensure(count)) || (r = en->seeds64.ensure(count)) || (r = en->seed32.ensure(count)) ||
+        (r = en->x397.ensure(count)) || (r = en->ps_l_array.ensure((size_t)src->n_l)) || (r = en->ps_rejected.ensure(PS_MAX_REJECTED)) ||
         (r = en->ps_count.ensure(2)))
         return r;
     if (n == 0) return TB200_OK;
@@ -638,14 +652,20 @@ int tb200_create_packets(tb200_engine *en, const tb200_packet_source *src) {
         P.energy = 1.0 / (double)n * factor / gamma;
     }
     en->e_typ = P.energy;
+    if (count == 0) return TB200_OK;
     {
-        const unsigned long long threads = ((unsigned long long)n + PS_CHUNK - 1) / PS_CHUNK;
-        packet_source_fill_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, en->stream>>>(P, en->in_r.p, en->in_nu.p, en->in_mu.p, en->in_energy.p,
+        const unsigned long long threads = ((unsigned long long)count + PS_CHUNK - 1) / PS_CHUNK;
+        packet_source_fill_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, en->stream>>>(P, (unsigned long long)lo, (unsigned long long)hi,
+                                                                                             en->in_r.p, en->in_nu.p, en->in_mu.p, en->in_energy.p,
                                                                                              en->seeds64.p);
         en->launches++;
         CK(cudaGetLastError());
     }
     return TB200_OK;
+}
+
+int tb200_create_packets(tb200_engine *en, const tb200_packet_source *src) {
+    return create_packets_range(en, src, 0, src ? src->n_packets : 0);
 }
 
 int tb200_download_packets(tb200_engine *en, double *radii, double *nus, double *mus, double *energies, int64_t *seeds) {
@@ -689,6 +709,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         CK(cudaMemsetAsync(en->ctrl.p, 0, (2 + tb::CNT_COUNT) * sizeof(unsigned long long), en->stream));
         CK(cudaMemsetAsync(en->error.p, 0, sizeof(int), en->stream));
         en->timing_valid = false;
+        en->est_unreduced = true;
     } else {
         CK(cudaMemsetAsync(en->ctrl.p, 0, sizeof(unsigned long long), en->stream));  // next_packet only
     }
@@ -1037,7 +1058,9 @@ int tb200_download(tb200_engine *en, tb200_outputs *o) {
 // of the outputs of range c-1 overlap (three streams; true overlap needs page-locked host buffers).
 // (pk == nullptr: the packets already lie in HBM -- uploaded earlier or generated by tb200_create_packets -- and only the
 //  per-packet outputs of range c-1 travel while range c computes)
-static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_outputs *o) {
+// log_on_device: the virtual-packet log stays in the engine's device buffer and only its count comes back (an engine group
+// copies the rows of all members straight into the caller's arrays afterwards).
+static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_outputs *o, bool log_on_device = false) {
     int r;
     const int64_t n = pk ? pk->n_packets : en->N;
     const bool tracking = o->last_interaction_type || (o->events && o->n_tracked_packets > 0) || (o->vlog_nus && o->vlog_capacity > 0);
@@ -1047,7 +1070,15 @@ static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_output
         if ((r = prepare_tracking(en, o))) return r;
         if ((r = launch_transport(en, 1))) return r;
         if ((r = tb200_sync(en))) return r;
-        return tb200_download(en, o);
+        if (!log_on_device) return tb200_download(en, o);
+        tb200_outputs q = *o;
+        q.vlog_nus = nullptr;
+        if ((r = tb200_download(en, &q))) return r;
+        o->counters = q.counters;
+        unsigned long long cnt = 0;
+        if (en->vlog_capacity > 0) CK(cudaMemcpy(&cnt, en->ctrl.p + 1, sizeof(cnt), cudaMemcpyDeviceToHost));
+        o->vlog_count = (int64_t)cnt;
+        return TB200_OK;
     }
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if (n > 2000000000LL) return fail(TB200_ERR_INVALID, "n_packets out of range");
@@ -1060,12 +1091,7 @@ static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_output
             return r;
     }
     if ((r = prepare_tracking(en, nullptr))) return r;
-    if (pk) {
-        const int64_t m = n < 65536 ? n : 65536;
-        double acc = 0.0;
-        for (int64_t i = 0; i < m; i++) acc += fabs(pk->initial_energies[i * (n / m)]);
-        en->e_typ = acc / (double)m;
-    }
+    if (pk) set_typical_energy(en, pk);
     std::vector<cudaEvent_t> ev_up(chunks), ev_k0(chunks), ev_k1(chunks);
     for (int c = 0; c < chunks; c++) { CK(cudaEventCreateWithFlags(&ev_up[c], cudaEventDisableTiming)); CK(cudaEventCreate(&ev_k0[c])); CK(cudaEventCreate(&ev_k1[c])); }
     int rc = TB200_OK;
@@ -1775,3 +1801,5 @@ int tb200_last_kernel_ms(tb200_engine *en, double *ms) {
 int64_t tb200_kernel_launches(tb200_engine *en) { return en ? en->launches : 0; }
 
 }  // extern "C"
+
+#include "group.cuh"  // engine groups: several engines driven from one call (needs tb200_engine's fields)

@@ -172,8 +172,9 @@ struct SourceParams {
     double beta;
 };
 
-// packets [i0, i1): radii, nus, mus, energies, seeds (any output pointer may be null)
-TB_HD void fill_chunk(const SourceParams &P, uint64_t i0, uint64_t i1, double *r, double *nu, double *mu, double *e, long long *seeds) {
+// packets [i0, i1): radii, nus, mus, energies, seeds (any output pointer may be null); packet i goes to element i - base
+TB_HD void fill_chunk(const SourceParams &P, uint64_t i0, uint64_t i1, double *r, double *nu, double *mu, double *e, long long *seeds,
+                      uint64_t base = 0) {
     Raw32 sr;
     sr.seek(P.origin, raw_index_of_output(i0, P.rejected, P.n_rej));
     Pcg64 gx[5], gm = P.origin;
@@ -185,11 +186,12 @@ TB_HD void fill_chunk(const SourceParams &P, uint64_t i0, uint64_t i1, double *r
         double xi[5];
         for (int j = 0; j < 5; j++) xi[j] = u64_to_double(pcg_next64(gx[j]));
         const double m = u64_to_double(pcg_next64(gm));
-        if (seeds) seeds[i] = (long long)lemire_value(x, P.rng_excl);
-        if (nu) nu[i] = blackbody_nu(xi[0], xi[1], xi[2], xi[3], xi[4], P.l_array, P.n_l, P.l_coef, P.k_b_t, P.h_planck);
-        if (mu) mu[i] = P.relativistic ? -P.beta + sqrt(P.beta * P.beta + 2 * P.beta * m + m) : sqrt(m);
-        if (r) r[i] = P.radius;
-        if (e) e[i] = P.energy;
+        const uint64_t k = i - base;
+        if (seeds) seeds[k] = (long long)lemire_value(x, P.rng_excl);
+        if (nu) nu[k] = blackbody_nu(xi[0], xi[1], xi[2], xi[3], xi[4], P.l_array, P.n_l, P.l_coef, P.k_b_t, P.h_planck);
+        if (mu) mu[k] = P.relativistic ? -P.beta + sqrt(P.beta * P.beta + 2 * P.beta * m + m) : sqrt(m);
+        if (r) r[k] = P.radius;
+        if (e) e[k] = P.energy;
     }
 }
 

@@ -67,6 +67,10 @@ class Engine:
         self._keep = []
 
     # ---- plumbing ----
+    def _api(self, name: str):
+        """The C function `tb200_<name>` that acts on this object's handle (an engine group maps it to `tb200_group_<name>`)."""
+        return getattr(self._lib, "tb200_" + name)
+
     def _check(self, code: int):
         if code == 0:
             return
@@ -95,8 +99,9 @@ class Engine:
         ctas_per_sm / park_min (0 = measured best for the kernel that will run; each kernel is compiled for its default CTAs
         per SM, so another ctas_per_sm only sizes the grid, at most to what fits), threads_per_cta (256 | 128), vol_min (24),
         refill_min (0 = 12 pooled classic / 8 otherwise), sort_packets (1), sort_bits (5), pipeline_chunks (8), pipeline_edges (1: the first and last
-        packet range of `run` are a quarter of the others), keep_opacity_tables (0).  An unknown name raises."""
-        self._check(self._lib.tb200_set_option(self._h, name.encode(), int(value)))
+        packet range of `run` are a quarter of the others), keep_opacity_tables (0).  An engine group also takes peer_access
+        (1; 0 stages every other member's slice of the collective through cudaMemcpyPeerAsync).  An unknown name raises."""
+        self._check(self._api("set_option")(self._h, name.encode(), int(value)))
 
     # ---- tables ----
     def set_model(self, *, r_inner, r_outer, time_explosion, electron_density, line_list_nu, tau_sobolev,
@@ -181,7 +186,7 @@ class Engine:
             keep.append(grid)
             c.spectrum_frequency_grid = _dptr(grid)
             c.n_grid = len(grid)
-        self._check(self._lib.tb200_set_model(self._h, C.byref(m), C.byref(c)))
+        self._check(self._api("set_model")(self._h, C.byref(m), C.byref(c)))
         self._model_shape = (m.n_lines, m.n_shells, int(c.n_grid))
         self._n_transitions = int(m.n_transitions)
         self._n_continua = int(m.n_continua) if continuum is not None else 0
@@ -294,7 +299,7 @@ class Engine:
         """The reference-facing call: host packet arrays in, host results out (`tb200_run`)."""
         pk, keep = self._packets_struct(initial_radii, initial_nus, initial_mus, initial_energies, packet_seeds)
         o, res = self._outputs_struct(pk.n_packets, **out_opts)
-        self._check(self._lib.tb200_run(self._h, C.byref(pk), C.byref(o)))
+        self._check(self._api("run")(self._h, C.byref(pk), C.byref(o)))
         self._n_packets = pk.n_packets
         return self._finish(o, res)
 
@@ -302,7 +307,7 @@ class Engine:
         """`tb200_run_resident`: the packets already in HBM (`upload_packets` / `create_packets`) through the same pipeline as
         `run` -- per-packet outputs stream back range by range while the next range computes."""
         o, res = self._outputs_struct(self._n_packets, **out_opts)
-        self._check(self._lib.tb200_run_resident(self._h, C.byref(o)))
+        self._check(self._api("run_resident")(self._h, C.byref(o)))
         return self._finish(o, res)
 
     def run_packets(self, packets, **out_opts):
@@ -311,8 +316,8 @@ class Engine:
 
     def upload_packets(self, initial_radii, initial_nus, initial_mus, initial_energies, packet_seeds):
         pk, keep = self._packets_struct(initial_radii, initial_nus, initial_mus, initial_energies, packet_seeds)
-        self._check(self._lib.tb200_upload_packets(self._h, C.byref(pk)))
-        self._check(self._lib.tb200_sync(self._h))  # host arrays may be released after this
+        self._check(self._api("upload_packets")(self._h, C.byref(pk)))
+        self._check(self._api("sync")(self._h))  # host arrays may be released after this
         self._n_packets = pk.n_packets
 
     def create_packets(self, n_packets: int, seed: int, radius: float, temperature: float, l_samples: int = 1000,
@@ -325,8 +330,8 @@ class Engine:
         src.l_array = l_array.ctypes.data_as(capi._pd); src.n_l = len(l_array); src.max_seed_val = int(max_seed_val)
         if beta is not None:  # BlackBodySimpleSourceRelativistic (black_body_relativistic.py:92-177)
             src.relativistic, src.beta = 1, float(beta)
-        self._check(self._lib.tb200_create_packets(self._h, C.byref(src)))
-        self._check(self._lib.tb200_sync(self._h))  # l_array may be released after this
+        self._check(self._api("create_packets")(self._h, C.byref(src)))
+        self._check(self._api("sync")(self._h))  # l_array may be released after this
         self._n_packets = int(n_packets)
 
     def download_packets(self):
@@ -374,7 +379,7 @@ class Engine:
         a.sobolev_coefficient = float((np.pi * e_esu**2) / (m_e * c))          # tau_sobolev.py:9-18
         a.c_einstein = float(4.0 * (np.pi * e_esu) ** 2 / (c * m_e))           # macroatom_line_transitions.py:9-11
         a.c, a.h = c, h
-        self._check(self._lib.tb200_set_atomic_data(self._h, C.byref(a)))
+        self._check(self._api("set_atomic_data")(self._h, C.byref(a)))
 
     def build_opacity(self, level_number_density, time_explosion, j_blues=None):
         """`tb200_build_opacity`: tau_Sobolev, beta_Sobolev and the normalised macro-atom probabilities of this iteration, built
@@ -387,7 +392,7 @@ class Engine:
             jb = _f64(j_blues)
             keep.append(jb)
             p.j_blues = _dptr(jb)
-        self._check(self._lib.tb200_build_opacity(self._h, C.byref(p)))
+        self._check(self._api("build_opacity")(self._h, C.byref(p)))
 
     def download_opacity(self, transition_probabilities=False):
         """The device-built tables in the reference's host layout: dict of tau_sobolev, beta_sobolev,
@@ -467,10 +472,10 @@ class Engine:
             raise ValueError("frequencies must be one-dimensional")
         lum = np.empty(len(freq))
         inup = np.empty((len(freq), int(points))) if want_intensities else None
-        self._check(self._lib.tb200_formal_integral(self._h, C.byref(p), _dptr(freq), len(freq), _dptr(lum),
+        self._check(self._api("formal_integral")(self._h, C.byref(p), _dptr(freq), len(freq), _dptr(lum),
                                                     _dptr(inup) if inup is not None else None))
         a, b = C.c_double(0.0), C.c_double(0.0)
-        self._check(self._lib.tb200_formal_integral_ms(self._h, C.byref(a), C.byref(b)))
+        self._check(self._api("formal_integral_ms")(self._h, C.byref(a), C.byref(b)))
         return dict(luminosity_densities=lum, intensities_nu_p=inup, interpolation_ms=a.value, integral_ms=b.value)
 
     # ---- estimator -> radiation field (SURVEY.md §8f rank 4) ----
@@ -546,3 +551,162 @@ class Engine:
         n = C.c_int64()
         self._check(self._lib.tb200_estimator_buffer(self._h, C.byref(p), C.byref(n)))
         return p.value, n.value
+
+
+class _MemberEngine(Engine):
+    """One member of an `EngineGroup`: an ordinary engine the group owns (every `Engine` call works on it; closing it only
+    drops this handle)."""
+
+    def __init__(self, group: "EngineGroup", handle: C.c_void_p, device: int):
+        self._lib = group._lib
+        self._h = handle
+        self.device = device
+        self._group = group  # keeps the owner alive
+        self._model_shape = None
+        self._n_packets = 0
+        self._n_continua = 0
+        self._keep = []
+
+    def close(self):
+        self._h = C.c_void_p()
+
+
+class EngineGroup(Engine):
+    """One MC iteration on several GPUs from one process (`tb200_group_*`): one engine per entry of `devices` (an id may
+    repeat: `[0, 0]` is two engines on device 0).  Same methods and result dicts as `Engine`; `run` / `run_resident` shard
+    the packets contiguously over the members (`parallel.shard_bounds`), sum the estimators on the devices and return
+    J_blue, Edotlu, the counters and every per-packet output bit-identical to one engine over the same packets (J, nu_bar,
+    the spectra and the luminosity sums to rounding).  `members` are the engines themselves."""
+
+    def __init__(self, devices):
+        devices = [int(d) for d in devices]
+        if not devices:
+            raise ValueError("an engine group needs at least one device")
+        self._lib = capi.load()
+        self._h = C.c_void_p()
+        self.members = []
+        self._check(self._lib.tb200_group_create((C.c_int * len(devices))(*devices), len(devices), C.byref(self._h)))
+        self.device = tuple(devices)
+        self._model_shape = None
+        self._n_packets = 0
+        self._n_continua = 0
+        self._keep = []
+        self.last_exact = None  # whether the last collective summed the fixed-point line accumulators
+        for i, d in enumerate(devices):
+            h = C.c_void_p()
+            self._check(self._lib.tb200_group_member(self._h, i, C.byref(h)))
+            self.members.append(_MemberEngine(self, h, d))
+
+    def _api(self, name: str):
+        return getattr(self._lib, "tb200_group_" + name)
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h:
+            for m in self.members:
+                m.close()
+            self._lib.tb200_group_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def shard_bounds(self, n: int):
+        """[(lo, hi)] of every member: the rule of `parallel.shard_bounds`."""
+        g = len(self.members)
+        return [(n * i // g, n * (i + 1) // g) for i in range(g)]
+
+    def _members_hold(self, n: int):
+        for m, (lo, hi) in zip(self.members, self.shard_bounds(n)):
+            m._n_packets = hi - lo
+        self._n_packets = n
+
+    # ---- tables ----
+    def set_model(self, **kw):
+        super().set_model(**kw)
+        for m in self.members:
+            m._model_shape, m._n_transitions, m._n_continua = self._model_shape, self._n_transitions, self._n_continua
+
+    def solve_radiation_field(self, **kw):
+        """On every member (each keeps the results resident for `build_opacity`); they are identical: member 0's."""
+        return [Engine.solve_radiation_field(m, **kw) for m in self.members][0]
+
+    def solve_source_function(self, **kw):
+        """On every member (the group's formal integral needs the tables on each); they are identical: member 0's."""
+        return [Engine.solve_source_function(m, **kw) for m in self.members][0]
+
+    def download_opacity(self, transition_probabilities=False):
+        return self.members[0].download_opacity(transition_probabilities)
+
+    def estimator_layout(self) -> dict:
+        return self.members[0].estimator_layout()
+
+    # ---- packets ----
+    def run(self, *args, **out_opts):
+        res = super().run(*args, **out_opts)
+        self._members_hold(self._n_packets)
+        self.last_exact = None
+        return res
+
+    def upload_packets(self, *args):
+        super().upload_packets(*args)
+        self._members_hold(self._n_packets)
+
+    def create_packets(self, n_packets: int, *args, **kw):
+        super().create_packets(n_packets, *args, **kw)
+        self._members_hold(int(n_packets))
+
+    def download_packets(self):
+        parts = [m.download_packets() for m in self.members]
+        return {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
+
+    def transport(self, zero_estimators: bool = True):
+        """`tb200_transport` on every member (members on one device one after the other); then call `allreduce`."""
+        busy = {}
+        for m in self.members:
+            if m.device in busy:
+                busy[m.device].sync()
+            m.transport(zero_estimators)
+            busy[m.device] = m
+
+    def sync(self):
+        self._check(self._lib.tb200_group_sync(self._h))
+
+    def allreduce(self) -> bool:
+        """`tb200_group_allreduce`: every member ends up with the summed estimators.  True when the fixed-point line
+        accumulators were summed (J_blue / Edotlu exact), False when the whole buffer was summed in f64."""
+        exact = C.c_int(0)
+        self._check(self._lib.tb200_group_allreduce(self._h, C.byref(exact)))
+        self.last_exact = bool(exact.value)
+        return self.last_exact
+
+    def allreduce_ms(self) -> float:
+        ms = C.c_double(0)
+        self._check(self._lib.tb200_group_allreduce_ms(self._h, C.byref(ms)))
+        return ms.value
+
+    def download(self, *, estimators=True, per_packet=True, buffers=None):
+        """After `transport` + `allreduce`: the estimators (member 0's copy) and the per-packet outputs of every member."""
+        res = self.members[0].download(estimators=estimators, per_packet=False, buffers=buffers)
+        if per_packet:
+            parts = [m.download(estimators=False, per_packet=True) for m in self.members]
+            for k in ("output_nus", "output_energies"):
+                res[k] = np.concatenate([p[k] for p in parts])
+        res["counters"] = self.counters()
+        return res
+
+    # ---- measurement ----
+    def counters(self) -> dict:
+        per = [m.counters() for m in self.members]
+        return {k: sum(c[k] for c in per) for k in capi.COUNTER_FIELDS}
+
+    def last_kernel_ms(self) -> float:
+        """The slowest member's transport kernel time."""
+        ran = [m for m in self.members if m._n_packets > 0]
+        if not ran:
+            raise EngineError("no member has transported packets")
+        return max(m.last_kernel_ms() for m in ran)
+
+    def kernel_launches(self) -> int:
+        return sum(m.kernel_launches() for m in self.members)
+
+    def _per_member(self, *_a, **_k):
+        raise EngineError("a group has one such buffer per member: use group.members[i]")
+
+    line_accumulators = finalize_line_estimators = estimator_buffer = _per_member

@@ -25,7 +25,7 @@ import logging
 
 import numpy as np
 
-from .engine import SIGMA_THOMSON, Engine, MacroAtomError, MonteCarloException  # noqa: F401 (re-exported)
+from .engine import SIGMA_THOMSON, Engine, EngineGroup, MacroAtomError, MonteCarloException  # noqa: F401 (re-exported)
 
 logger = logging.getLogger(__name__)
 
@@ -354,11 +354,13 @@ def _fused_sums(res, luminosity_nu_start, luminosity_nu_end):
 _engines = {}
 
 
-def get_engine(device: int = 0) -> Engine:
-    """One engine (device buffers persist across MC iterations) per device and process."""
-    if device not in _engines:
-        _engines[device] = Engine(device)
-    return _engines[device]
+def get_engine(device=0) -> Engine:
+    """One engine (device buffers persist across MC iterations) per device and process.  A sequence of device ids gives
+    one cached `EngineGroup` of them (an id may repeat: `[0, 0]` is two engines on device 0)."""
+    key = int(device) if isinstance(device, (int, np.integer)) else tuple(int(d) for d in device)
+    if key not in _engines:
+        _engines[key] = Engine(key) if isinstance(key, int) else EngineGroup(key)
+    return _engines[key]
 
 
 def montecarlo_transport_with_vpackets(
@@ -751,7 +753,8 @@ class MCTransportSolverB200:
     """Drop-in for ``MCTransportSolverClassic`` (modes/classic/solver.py:49-363): same constructor
     arguments, ``initialize_transport_state``, ``run`` and ``from_config``; the Numba main loop is
     replaced by the CUDA engine.  ``nthreads`` is accepted for signature compatibility (no host
-    threads are used); ``device`` selects the GPU of this process."""
+    threads are used); ``device`` selects the GPU of this process, or, as a list of ids, the `EngineGroup` that runs
+    each iteration on several GPUs from this process."""
 
     hdf_properties = ["transport_state"]
     hdf_name = "transport"
