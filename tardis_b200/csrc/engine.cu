@@ -56,6 +56,7 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 struct tb200_engine {
     int device = 0;
     int sm_count = 132;
+    size_t smem_optin = 227 * 1024;  // largest dynamic + static shared memory one CTA may opt in to (H100: 227 KiB)
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
     bool have_model = false;
@@ -194,6 +195,7 @@ int tb200_create(int device_id, tb200_engine **engine) {
         return fail(TB200_ERR_CUDA, why);
     }
     en->sm_count = prop.multiProcessorCount;
+    en->smem_optin = prop.sharedMemPerBlockOptin;
     *engine = en;
     return TB200_OK;
 }
@@ -853,6 +855,11 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         }
 #define TB_LAUNCH(KERNEL)                                                                                                  \
     do {                                                                                                                   \
+        /* refused here rather than by cudaFuncSetAttribute, whose error would stay pending and fail the next launch */   \
+        cudaFuncAttributes fa__;                                                                                           \
+        CK(cudaFuncGetAttributes(&fa__, KERNEL));                                                                          \
+        if (smem + fa__.sharedSizeBytes > en->smem_optin)                                                                  \
+            return fail(TB200_ERR_INVALID, "too many shells for the transport kernel's shared memory with this configuration"); \
         if (smem > 48 * 1024) CK(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
         int fit = 0;                                                                                                       \
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, KERNEL, threads, smem));                                    \
