@@ -345,6 +345,33 @@ int tb200_build_opacity(tb200_engine *engine, const tb200_plasma_state *plasma);
 int tb200_download_opacity(tb200_engine *engine, double *tau_sobolev /* [L,S] */, double *beta_sobolev /* [L,S] */,
                            double *stimulated_emission_factor /* [L,S] */, double *transition_probabilities /* [T,S] */);
 
+/* ---- the continuum mode's macro atom on the device ----
+ * Replaces steps 2-3 of ContinuumMacroAtomSolver._solve_next_macroatom_iteration (opacities/macro_atom/macroatom_solver.py:1648-1662):
+ * create_absorbing_probs (opacities/macro_atom/absorbing_markov_chain.py:19-134), which solves (I - Q) X = diag(1 - rowsum Q)
+ * per shell with scipy's splu, and the normalisation of the deactivating rows (internal rows zeroed; pandas' Kahan group sum
+ * per source block, NaN -> 0).  Usage: tb200_set_model in continuum mode with absorbing_markov_probabilities == NULL (or
+ * transition_probabilities == NULL) leaves the macro atom pending -- transport refuses to run -- and then every iteration
+ * tb200_build_absorbing_markov writes X (as the running sums the kernels read) and the normalised deactivation table into
+ * HBM.  Rows must be grouped by source as the model's macro_block_edge_index says (block b holds the rows of state b).
+ * Refused, before anything is allocated: an index out of range, rows not grouped as the block edges say, a table that does
+ * not fit on the device.  A chain that is not absorbing (a pivot <= 0 or not finite: splu's "singular matrix") is an error
+ * that names the shell and the state; the macro atom then stays pending.  See tardis_b200/csrc/markov_build.cuh. */
+typedef struct {
+    int64_t n_transitions;                       /* T, as in the model */
+    const double *transition_probabilities;      /* normalised (macroatom_solver.py:709-739): (row, shell) at
+                                                    [t*tp_transition_stride + s*tp_shell_stride] */
+    int64_t tp_transition_stride, tp_shell_stride;
+    const int64_t *source_level_idx, *destination_level_idx, *transition_type; /* [T]; rows with type >= 0 are internal.
+                                                    transition_type must equal the model's (the transport reads the rows by it);
+                                                    destination_level_idx is read for the internal rows only */
+    int64_t n_states;                            /* max(source_level_idx) + 1 */
+} tb200_markov_input;
+int tb200_build_absorbing_markov(tb200_engine *engine, const tb200_markov_input *input);
+/* X [S, n_states, n_states] as create_absorbing_probs returns it, and the normalised deactivation table [T,S] the transport
+ * reads; either pointer may be NULL.  Needs the option keep_opacity_tables = 1 before tb200_build_absorbing_markov (the
+ * kernels turn both tables into running sums in place). */
+int tb200_download_absorbing_markov(tb200_engine *engine, double *matrix, double *deactivating);
+
 /* ---- measurement ---- */
 int tb200_last_kernel_ms(tb200_engine *engine, double *ms);          /* CUDA-event time of the last tb200_transport kernel */
 int tb200_get_counters(tb200_engine *engine, tb200_counters *counters);
@@ -392,6 +419,7 @@ int tb200_group_set_option(tb200_group *group, const char *name, int64_t value);
 int tb200_group_set_model(tb200_group *group, const tb200_model *model, const tb200_config *config);
 int tb200_group_set_atomic_data(tb200_group *group, const tb200_atomic_data *atomic);
 int tb200_group_build_opacity(tb200_group *group, const tb200_plasma_state *plasma);
+int tb200_group_build_absorbing_markov(tb200_group *group, const tb200_markov_input *input); /* every member, bit-identical tables */
 int tb200_group_upload_packets(tb200_group *group, const tb200_packets *packets);
 int tb200_group_create_packets(tb200_group *group, const tb200_packet_source *source);
 int tb200_group_run(tb200_group *group, const tb200_packets *packets, tb200_outputs *outputs);

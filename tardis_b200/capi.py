@@ -16,11 +16,12 @@ EXPORTED_SYMBOLS = [
     "tb200_create_packets", "tb200_download_packets", "tb200_get_estimator_layout", "tb200_solve_radiation_field",
     "tb200_set_atomic_data", "tb200_build_opacity", "tb200_download_opacity",
     "tb200_line_accumulators", "tb200_finalize_line_estimators", "tb200_run_resident", "tb200_solve_source_function",
-    "tb200_formal_integral", "tb200_formal_integral_ms",
+    "tb200_formal_integral", "tb200_formal_integral_ms", "tb200_build_absorbing_markov", "tb200_download_absorbing_markov",
     "tb200_group_create", "tb200_group_destroy", "tb200_group_size", "tb200_group_member", "tb200_group_set_option",
     "tb200_group_set_model", "tb200_group_set_atomic_data", "tb200_group_build_opacity", "tb200_group_upload_packets",
     "tb200_group_create_packets", "tb200_group_run", "tb200_group_run_resident", "tb200_group_sync", "tb200_group_allreduce",
     "tb200_group_allreduce_ms", "tb200_group_formal_integral", "tb200_group_formal_integral_ms",
+    "tb200_group_build_absorbing_markov",
 ]
 
 
@@ -124,6 +125,15 @@ class PlasmaState(C.Structure):
     _fields_ = [("level_number_density", _pd), ("time_explosion", C.c_double), ("j_blues", _pd)]
 
 
+class MarkovInput(C.Structure):
+    """tb200_markov_input"""
+    _fields_ = [
+        ("n_transitions", C.c_int64), ("transition_probabilities", _pd), ("tp_transition_stride", C.c_int64),
+        ("tp_shell_stride", C.c_int64), ("source_level_idx", _pi), ("destination_level_idx", _pi), ("transition_type", _pi),
+        ("n_states", C.c_int64),
+    ]
+
+
 class Packets(C.Structure):
     _fields_ = [
         ("n_packets", C.c_int64), ("initial_radii", _pd), ("initial_nus", _pd), ("initial_mus", _pd),
@@ -211,6 +221,9 @@ def load(build_if_missing: bool = True):
     lib.tb200_solve_source_function.argtypes = [E, C.POINTER(SourceFunctionParams), _pd, _pd, _pd, _pd, C.POINTER(C.c_int32)]
     lib.tb200_formal_integral.argtypes = [E, C.POINTER(FormalIntegralParams), _pd, C.c_int64, _pd, _pd]
     lib.tb200_formal_integral_ms.argtypes = [E, _pd, _pd]
+    lib.tb200_build_absorbing_markov.argtypes = [E, C.POINTER(MarkovInput)]
+    lib.tb200_download_absorbing_markov.argtypes = [E, _pd, _pd]
+    lib.tb200_group_build_absorbing_markov.argtypes = [E, C.POINTER(MarkovInput)]
     lib.tb200_group_create.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(E)]
     lib.tb200_group_destroy.argtypes = [E]
     lib.tb200_group_destroy.restype = None
@@ -235,6 +248,7 @@ def load(build_if_missing: bool = True):
                  "tb200_set_atomic_data", "tb200_build_opacity", "tb200_download_opacity", "tb200_line_accumulators",
                  "tb200_finalize_line_estimators", "tb200_run_resident",
                  "tb200_solve_source_function", "tb200_formal_integral", "tb200_formal_integral_ms",
+                 "tb200_build_absorbing_markov", "tb200_download_absorbing_markov",
                  *(n for n in EXPORTED_SYMBOLS if n.startswith("tb200_group_") and n != "tb200_group_destroy")):
         getattr(lib, name).restype = C.c_int
     _lib = lib

@@ -17,6 +17,7 @@
 #include "radfield.cuh"
 #include "opacity_build.cuh"
 #include "formal_integral.cuh"
+#include "markov_build.cuh"
 
 namespace {
 
@@ -106,6 +107,11 @@ struct tb200_engine {
     long long k_packet_idx = -1;
     DBuf<double> t_e, bf_thr, pi_min, pi_max, x_sect, phot_nus, ff_factor, chi_bf_t, emiss_t, markov_cum;
     DBuf<int> pi_refs, pi_act;
+    // continuum macro atom built on the device (markov_build.cuh)
+    bool markov_pending = false;    // tb200_set_model got no absorbing_markov_probabilities / transition_probabilities
+    DBuf<double> mk_p_t, mk_q, mk_r, mk_c, mk_keep;  // normalised input [S][tpad]; q [S][n]; pivot row / column; kept X
+    DBuf<int> mk_type, mk_dest, mk_err;
+    int mk_keep_n = 0;              // n of the kept X (0: none)
     // global frequency bins of the bound-free opacity / estimators (continuum_bins.cuh)
     int cont_bins = 0, cb_n_gkeys = 0;
     long long cb_gkey_min = 0;
@@ -209,6 +215,8 @@ void tb200_destroy(tb200_engine *en) {
     en->t_e.release(); en->bf_thr.release(); en->pi_min.release(); en->pi_max.release(); en->x_sect.release(); en->phot_nus.release();
     en->cb_B.release(); en->cb_mom.release(); en->cont_lit.release(); en->cb_guide.release(); en->cb_nact.release(); en->cb_pos.release(); en->cb_chi_lin.release();
     en->ff_factor.release(); en->chi_bf_t.release(); en->emiss_t.release(); en->markov_cum.release(); en->pi_refs.release(); en->pi_act.release();
+    en->mk_p_t.release(); en->mk_q.release(); en->mk_r.release(); en->mk_c.release(); en->mk_keep.release();
+    en->mk_type.release(); en->mk_dest.release(); en->mk_err.release();
     en->line2macro.release(); en->block_edge.release(); en->ttype.release(); en->dest.release(); en->tline.release();
     en->est.release(); en->in_r.release(); en->in_nu.release(); en->in_mu.release(); en->in_energy.release();
     en->out_nu.release(); en->out_energy.release(); en->seeds64.release(); en->seed32.release(); en->x397.release(); en->ps_l_array.release(); en->ps_rejected.release(); en->ps_count.release();
@@ -339,6 +347,8 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     CK(cudaMemsetAsync(en->nu_line.p, 0, (en->lpad + TABLE_SLACK) * sizeof(double), en->stream));
     CK(cudaMemcpyAsync(en->nu_line.p, m->line_list_nu, L * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     en->opacity_pending = false;
+    en->markov_pending = false;
+    en->mk_keep_n = 0;
     if (m->tau_sobolev) {
         if ((r = upload_strided_table(en, m->tau_sobolev, L, S, m->tau_line_stride, m->tau_shell_stride, en->lpad, en->tau_t))) return r;
     } else {  // built on the device by tb200_build_opacity
@@ -360,10 +370,11 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
         if (m->transition_probabilities) {
             if ((r = upload_strided_table(en, m->transition_probabilities, en->T, S, m->tp_transition_stride, m->tp_shell_stride, en->tpad, en->tp_t))) return r;
         } else {
-            if (c->continuum_processes_enabled) return fail(TB200_ERR_INVALID, "the continuum mode's macro atom is not built on the device: pass transition_probabilities");
             if ((r = en->tp_t.ensure((size_t)S * en->tpad))) return r;
             CK(cudaMemsetAsync(en->tp_t.p, 0, (size_t)S * en->tpad * sizeof(double), en->stream));
-            en->opacity_pending = true;
+            // continuum mode: tb200_build_absorbing_markov writes the deactivation table; otherwise tb200_build_opacity
+            if (c->continuum_processes_enabled) en->markov_pending = true;
+            else en->opacity_pending = true;
         }
         en->have_macro = true;
         if ((r = upload_i64_as_i32(en, m->line2macro_level_upper, L, en->line2macro))) return r;
@@ -379,12 +390,12 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     // continuum (IIP mode) tables
     en->continuum = c->continuum_processes_enabled ? 1 : 0;
     if (en->continuum) {
-        if (c->line_interaction_type != 0 && (!m->transition_probabilities)) return fail(TB200_ERR_INVALID, "macro atom tables missing");
         if (!m->t_electrons || !m->phot_nus || !m->chi_bf || !m->x_sect || !m->emissivities || !m->photo_ion_block_references ||
             !m->photo_ion_nu_threshold_mins || !m->photo_ion_nu_threshold_maxs || !m->bf_threshold_list_nu || !m->ff_opacity_factor ||
-            !m->absorbing_markov_probabilities || !m->photo_ion_activation_idx)
+            !m->photo_ion_activation_idx)
             return fail(TB200_ERR_INVALID, "continuum tables missing");
-        if (m->n_continua < 0 || m->n_phot < 2 || m->n_markov < 1) return fail(TB200_ERR_INVALID, "bad continuum sizes");
+        if (m->n_continua < 0 || m->n_phot < 2 || (m->absorbing_markov_probabilities && m->n_markov < 1))
+            return fail(TB200_ERR_INVALID, "bad continuum sizes");
         en->n_continua = (int)m->n_continua; en->n_phot = (int)m->n_phot; en->phot_pad = round_up(en->n_phot, 32);
         en->n_activation = (int)m->n_activation; en->n_markov = (int)m->n_markov; en->k_packet_idx = m->k_packet_idx;
         for (int64_t k = 0; k < m->n_continua; k++)
@@ -408,13 +419,18 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
         if ((r = upload_strided_table(en, m->emissivities, en->n_phot, S, S, 1, en->phot_pad, en->emiss_t))) return r;
         if ((r = upload_i64_as_i32(en, m->photo_ion_block_references, m->n_continua + 1, en->pi_refs))) return r;
         if ((r = upload_i64_as_i32(en, m->photo_ion_activation_idx, m->n_activation, en->pi_act))) return r;
-        const size_t nm = (size_t)S * en->n_markov * en->n_markov;
-        if ((r = en->markov_cum.ensure(nm))) return r;
-        CK(cudaMemcpyAsync(en->markov_cum.p, m->absorbing_markov_probabilities, nm * sizeof(double), cudaMemcpyHostToDevice, en->stream));
-        const long long rows = (long long)S * en->n_markov;
-        tb::markov_cumsum_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, en->stream>>>(en->markov_cum.p, rows, en->n_markov);
-        en->launches++;
-        CK(cudaGetLastError());
+        if (m->absorbing_markov_probabilities) {
+            const size_t nm = (size_t)S * en->n_markov * en->n_markov;
+            if ((r = en->markov_cum.ensure(nm))) return r;
+            CK(cudaMemcpyAsync(en->markov_cum.p, m->absorbing_markov_probabilities, nm * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+            const long long rows = (long long)S * en->n_markov;
+            tb::markov_cumsum_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, en->stream>>>(en->markov_cum.p, rows, en->n_markov);
+            en->launches++;
+            CK(cudaGetLastError());
+        } else {  // built on the device by tb200_build_absorbing_markov
+            en->n_markov = 0;
+            en->markov_pending = true;
+        }
         // global frequency bins (continuum_bins.cuh): sorted union of the blocks, guide table, per-(shell, bin) linear chi_bf_tot
         {
             const tbc::HostBins hb = tbc::build_bins(m->phot_nus, en->n_phot, (const long long *)m->photo_ion_block_references, en->n_continua,
@@ -443,7 +459,7 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
         }
         if (c->line_interaction_type == 0) {
             // `scatter` lines with continuum: the macro atom is still needed for continuum events
-            if (!m->transition_probabilities || !m->macro_block_edge_index) return fail(TB200_ERR_INVALID, "macro atom tables missing");
+            if (!m->macro_block_edge_index) return fail(TB200_ERR_INVALID, "macro atom tables missing");
         }
     }
     // double-double prefix sums of tau along the line list, per shell (jump traces and virtual packets)
@@ -690,6 +706,9 @@ int tb200_download_packets(tb200_engine *en, double *radii, double *nus, double 
 static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bool last, int zero_estimators, cudaEvent_t ev_a, cudaEvent_t ev_b) {
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if (en->opacity_pending) return fail(TB200_ERR_NO_MODEL, "the opacity tables are pending: tb200_set_model got no tau_sobolev, call tb200_build_opacity");
+    if (en->markov_pending)
+        return fail(TB200_ERR_NO_MODEL, "the continuum macro atom is pending: tb200_set_model got no absorbing_markov_probabilities / "
+                                        "transition_probabilities, call tb200_build_absorbing_markov");
     CK(cudaSetDevice(en->device));
     const int S = en->S;
     const size_t row_words = (size_t)(en->lpad + 1) * 4;  // one shell's row of the difference arrays
@@ -1774,6 +1793,157 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
         CK(cudaMemcpyAsync(tp, en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
     }
+    return TB200_OK;
+}
+
+// ---- continuum macro atom on the device (markov_build.cuh) ----------------------------------------------------------
+// Everything is checked on the host before anything is allocated or launched, so a refused call leaves the engine as it was.
+static int check_markov_input(tb200_engine *en, const tb200_markov_input *in, std::vector<long long> &edges) {
+    if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
+    if (!en->continuum) return fail(TB200_ERR_INVALID, "tb200_build_absorbing_markov needs a continuum-mode model");
+    if (!in->transition_probabilities || !in->source_level_idx || !in->destination_level_idx || !in->transition_type)
+        return fail(TB200_ERR_INVALID, "absorbing Markov chain: an input array is NULL");
+    if (in->n_transitions != en->T) return fail(TB200_ERR_INVALID, "absorbing Markov chain: n_transitions differs from the model's");
+    if (in->tp_transition_stride < 0 || in->tp_shell_stride < 0) return fail(TB200_ERR_INVALID, "negative strides are not supported");
+    const int64_t T = in->n_transitions, n = in->n_states;
+    // the model's block edges (uploaded as int32 by tb200_set_model)
+    edges.assign((size_t)en->n_blocks + 1, 0);
+    {
+        std::vector<int> e32((size_t)en->n_blocks + 1);
+        CK(cudaMemcpy(e32.data(), en->block_edge.p, e32.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        for (size_t b = 0; b < e32.size(); b++) edges[b] = e32[b];
+    }
+    if (edges[0] != 0 || edges[(size_t)en->n_blocks] != T)
+        return fail(TB200_ERR_INVALID, "absorbing Markov chain: macro_block_edge_index must cover every row");
+    int64_t max_src = -1;
+    for (int64_t t = 0; t < T; t++) {
+        const int64_t a = in->source_level_idx[t];
+        if (a < 0 || a >= en->n_blocks) return fail(TB200_ERR_INVALID, "absorbing Markov chain: source_level_idx out of range at row " + std::to_string(t));
+        max_src = std::max(max_src, a);
+    }
+    if (n != max_src + 1) return fail(TB200_ERR_INVALID, "absorbing Markov chain: n_states must be max(source_level_idx) + 1");
+    for (int64_t b = 0; b < en->n_blocks; b++)
+        for (long long t = edges[(size_t)b]; t < edges[(size_t)b + 1]; t++)
+            if (in->source_level_idx[t] != b)
+                return fail(TB200_ERR_INVALID, "absorbing Markov chain: row " + std::to_string(t) + " has source " +
+                                                   std::to_string(in->source_level_idx[t]) + " but lies in block " + std::to_string(b) +
+                                                   " of macro_block_edge_index");
+    {  // the transport reads the rows by the model's types: the chain must be built from the same ones
+        std::vector<int> tt32((size_t)(T > 0 ? T : 1));
+        CK(cudaMemcpy(tt32.data(), en->ttype.p, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost));
+        for (int64_t t = 0; t < T; t++)
+            if (in->transition_type[t] != tt32[(size_t)t])
+                return fail(TB200_ERR_INVALID, "absorbing Markov chain: transition_type differs from the model's at row " + std::to_string(t));
+    }
+    for (int64_t t = 0; t < T; t++)
+        if (in->transition_type[t] >= 0 && (in->destination_level_idx[t] < 0 || in->destination_level_idx[t] >= n))
+            return fail(TB200_ERR_INVALID, "absorbing Markov chain: destination_level_idx out of range at internal row " + std::to_string(t));
+    // the table: [S, n, n] doubles (twice with keep_opacity_tables), indices of the kernels' grids
+    if (n > 65535 || en->S > 65535 || (long long)n * en->S >= INT_MAX)
+        return fail(TB200_ERR_INVALID, "absorbing Markov chain: " + std::to_string(n) + " states x " + std::to_string(en->S) + " shells do not fit the solver");
+    const double need = (double)en->S * n * n * 8.0 * (en->keep_opacity_tables ? 2 : 1) +
+                        8.0 * ((double)en->S * (en->tpad + 3.0 * n) + TABLE_SLACK) + 8.0 * en->T;  // + input table, q / r / c, type / dest
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const double have = (double)free_b + 8.0 * ((double)en->markov_cum.n + en->mk_keep.n + en->mk_p_t.n + en->mk_q.n + en->mk_r.n + en->mk_c.n) +
+                        4.0 * ((double)en->mk_type.n + en->mk_dest.n);
+    if (need > have)
+        return fail(TB200_ERR_INVALID, "absorbing Markov chain: the table needs " + std::to_string(need / 1e9) + " GB, " +
+                                           std::to_string(have / 1e9) + " GB are free on the device");
+    return TB200_OK;
+}
+
+int tb200_build_absorbing_markov(tb200_engine *en, const tb200_markov_input *in) {
+    if (!en || !in) return fail(TB200_ERR_INVALID, "bad argument");
+    CK(cudaSetDevice(en->device));
+    std::vector<long long> edges;
+    int r;
+    if ((r = check_markov_input(en, in, edges))) return r;
+    const int S = en->S, n = (int)in->n_states;
+    cudaStream_t st = en->stream;
+    en->markov_pending = true;  // until the build below has finished
+    en->mk_keep_n = 0;
+    if ((r = upload_strided_table(en, in->transition_probabilities, en->T, S, in->tp_transition_stride, in->tp_shell_stride, en->tpad, en->mk_p_t)) ||
+        (r = upload_i64_as_i32(en, in->transition_type, en->T, en->mk_type)) ||
+        (r = upload_i64_as_i32(en, in->destination_level_idx, en->T, en->mk_dest)))
+        return r;
+    const size_t nm = (size_t)S * n * n, sn = (size_t)S * n;
+    if ((r = en->markov_cum.ensure(nm)) || (r = en->mk_q.ensure(sn)) || (r = en->mk_r.ensure(sn)) || (r = en->mk_c.ensure(sn)) ||
+        (r = en->mk_err.ensure(1)))
+        return r;
+    if (en->keep_opacity_tables && (r = en->mk_keep.ensure(nm))) return r;
+    const int no_error = INT_MAX;
+    CK(cudaMemcpyAsync(en->mk_err.p, &no_error, sizeof(int), cudaMemcpyHostToDevice, st));
+    double *A = en->markov_cum.p;
+    CK(cudaMemsetAsync(A, 0, nm * sizeof(double), st));
+    tbm::markov_assemble_kernel<<<(unsigned)((sn + 127) / 128), 128, 0, st>>>(en->mk_p_t.p, en->tpad, en->block_edge.p, en->mk_type.p,
+                                                                            en->mk_dest.p, n, S, A, en->mk_q.p);
+    tbm::markov_identity_minus_kernel<<<(unsigned)((nm + 255) / 256), 256, 0, st>>>(A, n, (long long)nm);
+    en->launches += 2;
+    CK(cudaGetLastError());
+    if (n <= tbm::SMEM_MAX_N) {
+        const size_t smem = ((size_t)n * n + 2 * (size_t)n) * sizeof(double);
+        CK(cudaFuncSetAttribute(tbm::markov_solve_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        tbm::markov_solve_smem_kernel<<<S, 256, smem, st>>>(A, n, S, en->mk_err.p);
+        en->launches++;
+        CK(cudaGetLastError());
+    } else {
+        const dim3 grid((unsigned)((n + 127) / 128), (unsigned)n, (unsigned)S);
+        for (int k = 0; k < n; k++) {
+            tbm::markov_pivot_kernel<<<(unsigned)((sn + 255) / 256), 256, 0, st>>>(A, n, S, k, en->mk_r.p, en->mk_c.p, en->mk_err.p);
+            tbm::markov_update_kernel<<<grid, 128, 0, st>>>(A, n, k, en->mk_r.p, en->mk_c.p);
+        }
+        en->launches += 2LL * n;
+        CK(cudaGetLastError());
+    }
+    int err = no_error;
+    CK(cudaMemcpyAsync(&err, en->mk_err.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (err != no_error)
+        return fail(TB200_ERR_INVALID, "absorbing Markov chain: I - Q is singular in shell " + std::to_string(err % S) + " at state " +
+                                           std::to_string(err / S) + " (a pivot <= 0 or not finite: the chain is not absorbing)");
+    tbm::markov_scale_kernel<<<(unsigned)((nm + 255) / 256), 256, 0, st>>>(A, en->mk_q.p, n, S, en->keep_opacity_tables ? en->mk_keep.p : nullptr);
+    const long long rows = (long long)sn;
+    tb::markov_cumsum_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(A, rows, n);
+    const long long nb = (long long)en->n_blocks * S;
+    tbm::markov_deactivation_kernel<<<(unsigned)((nb + 127) / 128), 128, 0, st>>>(en->mk_p_t.p, en->tpad, en->block_edge.p, en->n_blocks,
+                                                                                en->mk_type.p, S, en->tp_t.p);
+    en->launches += 3;
+    CK(cudaGetLastError());
+    if (en->keep_opacity_tables) {
+        if ((r = en->op_tp_norm_t.ensure((size_t)S * en->tpad))) return r;
+        CK(cudaMemcpyAsync(en->op_tp_norm_t.p, en->tp_t.p, (size_t)S * en->tpad * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        en->mk_keep_n = n;
+    }
+    if ((r = finish_opacity_tables(en))) return r;
+    CK(cudaStreamSynchronize(st));
+    en->n_markov = n;
+    en->markov_pending = false;
+    return TB200_OK;
+}
+
+int tb200_download_absorbing_markov(tb200_engine *en, double *matrix, double *deactivating) {
+    if (!en) return fail(TB200_ERR_INVALID, "bad argument");
+    if (!en->have_model || !en->continuum || en->markov_pending) return fail(TB200_ERR_NO_MODEL, "no absorbing Markov chain on the device");
+    CK(cudaSetDevice(en->device));
+    if (en->mk_keep_n == 0)
+        return fail(TB200_ERR_INVALID, "the chain was not kept: set the option keep_opacity_tables = 1 before tb200_build_absorbing_markov");
+    cudaStream_t st = en->stream;
+    const int S = en->S;
+    if (matrix) {
+        const size_t nm = (size_t)S * en->mk_keep_n * en->mk_keep_n;
+        CK(cudaMemcpyAsync(matrix, en->mk_keep.p, nm * sizeof(double), cudaMemcpyDeviceToHost, st));
+    }
+    if (deactivating) {
+        int r;
+        if ((r = en->staging.ensure((size_t)en->T * S))) return r;
+        const long long cells = (long long)en->T * S;
+        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(en->op_tp_norm_t.p, en->T, S, en->tpad, en->staging.p);
+        en->launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(deactivating, en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
     return TB200_OK;
 }
 

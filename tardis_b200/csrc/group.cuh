@@ -363,6 +363,11 @@ int tb200_group_build_opacity(tb200_group *g, const tb200_plasma_state *plasma) 
     });
 }
 
+int tb200_group_build_absorbing_markov(tb200_group *g, const tb200_markov_input *input) {
+    if (!g) return fail(TB200_ERR_INVALID, "bad argument");
+    return group_parallel(g, nullptr, [&](int i) { return tb200_build_absorbing_markov(g->m[(size_t)i], input); });
+}
+
 int tb200_group_upload_packets(tb200_group *g, const tb200_packets *pk) {
     if (!g || !pk) return fail(TB200_ERR_INVALID, "bad argument");
     if (pk->n_packets < 0 || pk->n_packets > 2000000000LL) return fail(TB200_ERR_INVALID, "n_packets out of range");

@@ -64,6 +64,7 @@ class Engine:
         self._model_shape = None
         self._n_packets = 0
         self._n_continua = 0
+        self._n_markov = 0
         self._keep = []
 
     # ---- plumbing ----
@@ -114,7 +115,9 @@ class Engine:
                   luminosity_nu_end=np.inf):
         """`continuum`: object with the IIP fields of OpacityStateNumbaIIP (bf_threshold_list_nu,
         photo_ion_nu_threshold_mins/maxs, photo_ion_block_references, chi_bf, x_sect, phot_nus, ff_opacity_factor,
-        emissivities, photo_ion_activation_idx, k_packet_idx, absorbing_markov_probabilities) -> IIP mode."""
+        emissivities, photo_ion_activation_idx, k_packet_idx, absorbing_markov_probabilities) -> IIP mode.
+        absorbing_markov_probabilities = None (or transition_probabilities = None) leaves the continuum macro atom pending
+        until `build_absorbing_markov`."""
         keep = []
         m = capi.Model()
         r_inner, r_outer, n_e, nu = _f64(r_inner), _f64(r_outer), _f64(electron_density), _f64(line_list_nu)
@@ -155,7 +158,8 @@ class Engine:
             te = _f64(t_electrons)
             cf = {k: _f64(getattr(continuum, k)) for k in (
                 "bf_threshold_list_nu", "photo_ion_nu_threshold_mins", "photo_ion_nu_threshold_maxs", "chi_bf", "x_sect",
-                "phot_nus", "ff_opacity_factor", "emissivities", "absorbing_markov_probabilities")}
+                "phot_nus", "ff_opacity_factor", "emissivities", "absorbing_markov_probabilities")
+                if k != "absorbing_markov_probabilities" or getattr(continuum, k) is not None}
             ci = {k: _i64(getattr(continuum, k)) for k in ("photo_ion_block_references", "photo_ion_activation_idx")}
             keep += [te] + list(cf.values()) + list(ci.values())
             m.t_electrons = _dptr(te)
@@ -166,9 +170,10 @@ class Engine:
                 setattr(m, k, _iptr(v))
             m.n_activation = len(ci["photo_ion_activation_idx"])
             m.k_packet_idx = int(continuum.k_packet_idx)
-            if cf["absorbing_markov_probabilities"].ndim != 3:
-                raise ValueError("absorbing_markov_probabilities must be [n_shells, n, n]")
-            m.n_markov = cf["absorbing_markov_probabilities"].shape[1]
+            if "absorbing_markov_probabilities" in cf:  # otherwise built on the device by build_absorbing_markov
+                if cf["absorbing_markov_probabilities"].ndim != 3:
+                    raise ValueError("absorbing_markov_probabilities must be [n_shells, n, n]")
+                m.n_markov = cf["absorbing_markov_probabilities"].shape[1]
         c = capi.Config()
         c.continuum_processes_enabled = int(continuum is not None)
         c.enable_full_relativity = int(bool(enable_full_relativity))
@@ -406,6 +411,49 @@ class Engine:
             out["transition_probabilities"] = tp
         return out
 
+    # ---- the continuum macro atom on the device ----
+    def build_absorbing_markov(self, transition_probabilities, source_level_idx, destination_level_idx, transition_type,
+                               n_states=None):
+        """`tb200_build_absorbing_markov`: the absorbing-Markov-chain table X [S, n, n] and the normalised deactivation table
+        of this iteration, built in HBM from the normalised transition probabilities [T, S] (may be a strided view) and the
+        rows' source / destination state and type (create_absorbing_probs + the second normalisation of the reference's
+        ContinuumMacroAtomSolver).  n_states defaults to max(source_level_idx) + 1."""
+        tp = np.asarray(transition_probabilities, dtype=np.float64)
+        if tp.ndim != 2:
+            raise ValueError("transition_probabilities must be [n_transitions, n_shells]")
+        if any(s < 0 or s % 8 for s in tp.strides):
+            tp = np.ascontiguousarray(tp)
+        src, dst, tt = _i64(source_level_idx), _i64(destination_level_idx), _i64(transition_type)
+        if not (len(src) == len(dst) == len(tt) == tp.shape[0]):
+            raise ValueError("source_level_idx, destination_level_idx and transition_type need one entry per row")
+        if tp.shape[1] != self._model_shape[1]:
+            raise ValueError("transition_probabilities must have one column per shell of the model")
+        keep = [tp, src, dst, tt]
+        m = capi.MarkovInput()
+        m.n_transitions = tp.shape[0]
+        m.transition_probabilities = _dptr(tp)
+        m.tp_transition_stride, m.tp_shell_stride = tp.strides[0] // 8, tp.strides[1] // 8
+        m.source_level_idx, m.destination_level_idx, m.transition_type = _iptr(src), _iptr(dst), _iptr(tt)
+        m.n_states = int(src.max()) + 1 if n_states is None else int(n_states)
+        self._check(self._api("build_absorbing_markov")(self._h, C.byref(m)))
+        self._n_markov = int(m.n_states)
+        del keep
+
+    def download_absorbing_markov(self, matrix=True, deactivating=True):
+        """The device-built tables in the reference's host layout: dict of absorbing_markov_probabilities [S, n, n] and the
+        normalised deactivating transition_probabilities [T, S]; needs the option keep_opacity_tables = 1 before the build."""
+        _, S, _ = self._model_shape
+        n = self._n_markov
+        out = {}
+        if matrix:
+            out["absorbing_markov_probabilities"] = np.empty((S, n, n))
+        if deactivating:
+            out["transition_probabilities"] = np.empty((self._n_transitions, S))
+        self._check(self._lib.tb200_download_absorbing_markov(
+            self._h, _dptr(out["absorbing_markov_probabilities"]) if matrix else None,
+            _dptr(out["transition_probabilities"]) if deactivating else None))
+        return out
+
     # ---- formal-integral source function (SURVEY.md §8f rank 4) ----
     def solve_source_function(self, *, time_explosion, time_of_simulation, volume, wavelength_cm, lines_lower_level_idx,
                               lines_upper_level_idx, n_levels, estimators=None, c=2.99792458e10, tolerance=0.0, max_iterations=0,
@@ -565,6 +613,7 @@ class _MemberEngine(Engine):
         self._model_shape = None
         self._n_packets = 0
         self._n_continua = 0
+        self._n_markov = 0
         self._keep = []
 
     def close(self):
@@ -590,6 +639,7 @@ class EngineGroup(Engine):
         self._model_shape = None
         self._n_packets = 0
         self._n_continua = 0
+        self._n_markov = 0
         self._keep = []
         self.last_exact = None  # whether the last collective summed the fixed-point line accumulators
         for i, d in enumerate(devices):
@@ -633,6 +683,15 @@ class EngineGroup(Engine):
 
     def download_opacity(self, transition_probabilities=False):
         return self.members[0].download_opacity(transition_probabilities)
+
+    def build_absorbing_markov(self, *args, **kw):
+        """On every member (`tb200_group_build_absorbing_markov`); the members' tables are bit-identical."""
+        super().build_absorbing_markov(*args, **kw)
+        for m in self.members:
+            m._n_markov = self._n_markov
+
+    def download_absorbing_markov(self, matrix=True, deactivating=True):
+        return self.members[0].download_absorbing_markov(matrix, deactivating)
 
     def estimator_layout(self) -> dict:
         return self.members[0].estimator_layout()

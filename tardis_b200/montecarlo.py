@@ -25,6 +25,7 @@ import logging
 
 import numpy as np
 
+from . import macro_atom
 from .engine import SIGMA_THOMSON, Engine, EngineGroup, MacroAtomError, MonteCarloException  # noqa: F401 (re-exported)
 
 logger = logging.getLogger(__name__)
@@ -480,6 +481,9 @@ def montecarlo_transport(
     cfg = montecarlo_configuration
     eng = engine or get_engine()
     o = opacity_state_numba
+    # the X that tardis_b200.macro_atom.create_absorbing_probs returned: rebuilt in HBM from its [T, S] input, not uploaded
+    rebuild = macro_atom.built_inputs(getattr(o, "absorbing_markov_probabilities", None), o.transition_type)
+    montecarlo_transport.last_markov_rebuilt = rebuild is not None
     eng.set_model(
         r_inner=_value(geometry_state_numba.r_inner), r_outer=_value(geometry_state_numba.r_outer),
         time_explosion=float(_value(time_explosion)),
@@ -492,9 +496,11 @@ def montecarlo_transport(
                                  else np.ascontiguousarray(_value(spectrum_frequency_grid), dtype=np.float64)),
         enable_full_relativity=True,
         disable_line_scattering=bool(cfg.DISABLE_LINE_SCATTERING), sigma_thomson=sigma_thomson,
-        continuum=o, t_electrons=o.t_electrons,
+        continuum=o if rebuild is None else macro_atom.WithoutMatrix(o), t_electrons=o.t_electrons,
         luminosity_nu_start=float(_value(luminosity_nu_start)), luminosity_nu_end=float(_value(luminosity_nu_end)),
     )
+    if rebuild is not None:
+        eng.build_absorbing_markov(**rebuild)
     n_cont = len(o.bf_threshold_list_nu)
     if tuple(n_levels_bf_species_by_n_cells_tuple) not in ((n_cont, len(o.electron_density)), (0, 0)):
         logger.debug("n_levels_bf_species_by_n_cells_tuple %s differs from the continuum tables (%d, %d)",

@@ -340,6 +340,98 @@ def add_continuum(model: Model, seed: int = MODEL_SEED + 1, n_continua: int = 30
     return model
 
 
+@dataclass
+class ContinuumMacroAtom:
+    """What create_absorbing_probs takes (opacities/macro_atom/absorbing_markov_chain.py:19-56): the normalised probabilities
+    and the rows' metadata.  Rows are grouped by source state; block b = state b."""
+
+    transition_probabilities: np.ndarray  # f64[T, S], normalised per source block
+    source_level_idx: np.ndarray          # i64[T]
+    destination_level_idx: np.ndarray     # i64[T] (internal rows: a state; deactivation rows: -1)
+    transition_type: np.ndarray           # i64[T]; >= 0 internal
+    macro_block_edge_index: np.ndarray    # i64[n_states + 1]
+    n_states: int
+
+
+def add_continuum_macro_atom(model: Model, seed: int = MODEL_SEED + 2, n_levels: int = 60, internal_rows: tuple[int, int] = (1, 12),
+                             deactivation_rows: tuple[int, int] = (1, 4), internal_share: tuple[float, float] = (0.3, 0.97),
+                             n_groups: int = 1, duplicate_fraction: float = 0.0, self_loop_fraction: float = 0.0,
+                             zero_blocks: int = 0, ill_conditioned_shell: int | None = None) -> ContinuumMacroAtom:
+    """A continuum macro atom with real internal rows for `model` (made IIP by `add_continuum` first): `n_levels` levels plus a
+    k-packet and an i-packet state.  Every state gets internal rows (internal down / up, type 0 / 1) to other states of its
+    group (states g, g + n_groups, ...: with n_groups > 1 no path joins two groups, so X has a block zero pattern) and
+    deactivation rows (line / bound-free / free-free emission for levels; k-packet: free-bound / free-free cooling and
+    adiabatic cooling; i-packet: photo-recombination emission), in random order inside the block.  Per (state, shell) the
+    internal rows carry a share drawn from `internal_share` (1 - 1e-6 everywhere in `ill_conditioned_shell`).
+    `duplicate_fraction` repeats the previous destination, `self_loop_fraction` points a row at its own state, `zero_blocks`
+    levels get all-zero probabilities.  The model's macro-atom tables become these rows, with the normalised probabilities
+    as transition_probabilities and absorbing_markov_probabilities = None (to be built by the engine); `add_continuum` and
+    the models it makes are unchanged."""
+    rng = np.random.default_rng(seed)
+    S, L = model.n_shells, model.n_lines
+    n_cont = len(model.continuum.bf_threshold_list_nu)
+    k_idx, i_idx, n_states = n_levels, n_levels + 1, n_levels + 2
+    members = [np.arange(g, n_states, n_groups) for g in range(n_groups)]
+    src, dst, ttype, tline, edges, share_rows = [], [], [], [], [0], []
+    for b in range(n_states):
+        group = members[b % n_groups]
+        rows = []
+        for _ in range(int(rng.integers(internal_rows[0], internal_rows[1] + 1))):
+            if rows and rng.random() < duplicate_fraction:
+                d = rows[-1][1]
+            elif rng.random() < self_loop_fraction or len(group) == 1:
+                d = b
+            else:
+                d = int(rng.choice(group[group != b]))
+            rows.append((int(rng.integers(0, 2)), d, 0))
+        for _ in range(int(rng.integers(deactivation_rows[0], deactivation_rows[1] + 1))):
+            if b == k_idx:
+                t = int(rng.choice([-20, -21, -4], p=[0.6, 0.35, 0.05]))
+            elif b == i_idx:
+                t = -7
+            else:
+                t = int(rng.choice([-1, -2, -3], p=[0.8, 0.15, 0.05]))
+            rows.append((t, -1, int(rng.integers(0, L - 1)) if t == -1 else (int(rng.integers(0, n_cont)) if t in (-2, -7, -20) else 0)))
+        for j in rng.permutation(len(rows)):
+            t, d, tl = rows[j]
+            src.append(b); ttype.append(t); dst.append(d); tline.append(tl)
+        edges.append(len(src))
+    src, dst, ttype, tline = (np.array(a, dtype=np.int64) for a in (src, dst, ttype, tline))
+    edges = np.array(edges, dtype=np.int64)
+    raw = rng.random((len(src), S)) + 0.05
+    share = rng.uniform(internal_share[0], internal_share[1], (n_states, S))
+    if ill_conditioned_shell is not None:
+        share[:, ill_conditioned_shell] = 1.0 - 1e-6
+    internal = ttype >= 0
+    probs = np.zeros_like(raw)
+    for b in range(n_states):
+        blk = slice(edges[b], edges[b + 1])
+        inn, out = internal[blk], ~internal[blk]
+        r = raw[blk]
+        part = np.zeros_like(r)
+        if inn.any() and out.any():
+            part[inn] = r[inn] / r[inn].sum(axis=0) * share[b]
+            part[out] = r[out] / r[out].sum(axis=0) * (1.0 - share[b])
+        else:
+            part = r / r.sum(axis=0)
+        probs[blk] = part
+    for b in rng.choice(n_levels, zero_blocks, replace=False) if zero_blocks else ():
+        probs[edges[b]:edges[b + 1]] = 0.0
+    probs = np.ascontiguousarray(probs)
+    model.macro = MacroAtomTables(
+        transition_probabilities=probs,
+        line2macro_level_upper=rng.integers(0, n_levels, L).astype(np.int64),
+        macro_block_edge_index=edges,
+        transition_type=ttype,
+        destination_level_id=dst,
+        transition_line_id=tline,
+    )
+    model.continuum.k_packet_idx = k_idx
+    model.continuum.photo_ion_activation_idx = np.full(len(model.continuum.photo_ion_activation_idx), i_idx, dtype=np.int64)
+    model.continuum.absorbing_markov_probabilities = None
+    return ContinuumMacroAtom(probs, src, dst, ttype, edges, n_states)
+
+
 def make_packets(
     n_packets: int,
     r_inner0: float,
