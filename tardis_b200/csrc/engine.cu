@@ -89,6 +89,7 @@ struct tb200_engine {
     DBuf<int> first_le;
     long long key_min = 0; int n_keys = 0;
     DBuf<int> macro_guide;             // [S][tpad] (classic macro atom)
+    DBuf<int2> macro_next, macro_entry;  // [T], [L] (classic macro atom)
     DBuf<unsigned long long> cnt_rep;  // [BULK_REPS][CNT_COUNT] rare-path counter replicas
     DBuf<double> bulk_rep;          // jump algorithm: [BULK_REPS][2 S] J / nu_bar replicas (zero between launches)
     double grid0 = 0, grid_last = 0, inv_dgrid = 0;
@@ -211,7 +212,7 @@ void tb200_destroy(tb200_engine *en) {
     cudaSetDevice(en->device);
     cudaStreamSynchronize(en->stream);
     en->r_inner.release(); en->r_outer.release(); en->n_e.release(); en->nu_line.release(); en->tau_t.release();
-    en->prefix.release(); en->first_le.release(); en->diff.release(); en->xfer.release(); en->bulk_rep.release(); en->cnt_rep.release(); en->macro_guide.release(); en->tp_t.release(); en->grid.release(); en->staging.release();
+    en->prefix.release(); en->first_le.release(); en->diff.release(); en->xfer.release(); en->bulk_rep.release(); en->cnt_rep.release(); en->macro_guide.release(); en->macro_next.release(); en->macro_entry.release(); en->tp_t.release(); en->grid.release(); en->staging.release();
     en->t_e.release(); en->bf_thr.release(); en->pi_min.release(); en->pi_max.release(); en->x_sect.release(); en->phot_nus.release();
     en->cb_B.release(); en->cb_mom.release(); en->cont_lit.release(); en->cb_guide.release(); en->cb_nact.release(); en->cb_pos.release(); en->cb_chi_lin.release();
     en->ff_factor.release(); en->chi_bf_t.release(); en->emiss_t.release(); en->markov_cum.release(); en->pi_refs.release(); en->pi_act.release();
@@ -308,6 +309,12 @@ static int finish_opacity_tables(tb200_engine *en) {
         CK(cudaGetLastError());
         if ((r = en->macro_guide.ensure((size_t)S * en->tpad))) return r;
         tb::macro_guide_kernel<<<(unsigned)((total + 127) / 128), 128, 0, en->stream>>>(en->tp_t.p, en->block_edge.p, en->n_blocks, S, en->tpad, en->macro_guide.p);
+        en->launches++;
+        CK(cudaGetLastError());
+        if ((r = en->macro_next.ensure((size_t)std::max(en->T, 1))) || (r = en->macro_entry.ensure((size_t)en->L))) return r;
+        const int n_items = std::max(en->T, en->L);
+        tb::macro_next_kernel<<<(unsigned)((n_items + 255) / 256), 256, 0, en->stream>>>(en->block_edge.p, en->ttype.p, en->dest.p, en->tline.p,
+            en->line2macro.p, en->n_blocks, en->T, en->L, en->macro_next.p, en->macro_entry.p);
         en->launches++;
         CK(cudaGetLastError());
         en->have_macro_guide = true;
@@ -797,6 +804,8 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         }
         P.cnt_rep = en->cnt_rep.p;
         P.macro_guide = (en->have_macro_guide && !en->continuum) ? en->macro_guide.p : nullptr;
+        P.macro_next = (en->have_macro_guide && !en->continuum) ? en->macro_next.p : nullptr;
+        P.macro_entry = (en->have_macro_guide && !en->continuum) ? en->macro_entry.p : nullptr;
         P.bulk_rep = en->bulk_rep.p; P.bulk_reps = BULK_REPS;
     }
     P.vol_min = en->vol_min;

@@ -45,6 +45,13 @@ enum Counter {
     CNT_MACRO_JUMPS, CNT_MACRO_SCANNED, CNT_VPACKETS, CNT_VPACKET_LINE_STEPS, CNT_CONT_EVENTS, CNT_BF_UPDATES, CNT_PROBES, CNT_COUNT
 };
 
+// Where a classic macro-atom transition leads, one int2 per transition (macro_next_kernel), independent of the shell:
+// {start, end} of the destination block for an internal jump (start >= 0), {MNEXT_EMIT, line} for an emission,
+// {MNEXT_BAD_LEVEL, 0} for an internal jump to a level outside the table, {MNEXT_BAD_TYPE, 0} for any other type.  The same
+// encoding, per line, gives the block that absorbing the line activates (macro_entry).  One load then gives a jump both
+// its outcome and the next block, where dest / ttype / tline and block_edge took two dependent loads.
+constexpr int MNEXT_EMIT = -1, MNEXT_BAD_LEVEL = -2, MNEXT_BAD_TYPE = -3;
+
 struct Event {  // == tb200_event
     long long packet_id, interaction_type, status, before_shell_id, after_shell_id, line_absorb_id, line_emit_id;
     double radius, before_nu, before_mu, before_energy, after_nu, after_mu, after_energy;
@@ -107,6 +114,8 @@ struct KParams {
     unsigned long long *counters;            // [CNT_COUNT]
     double grid0, grid_last, inv_dgrid;      // spectrum grid: first / last edge, 1 / (edge[1] - edge[0]) (binning guess only)
     const int *macro_guide;                  // [S][tpad] bracket table of the classic macro atom (macro_guide_kernel), or null
+    const int2 *macro_next, *macro_entry;    // [T] / [L] classic macro atom: where a transition leads / the block a line
+                                             //    activates (macro_next_kernel), or null in continuum mode
     unsigned long long *cnt_rep;             // [bulk_reps][CNT_COUNT] replicas of the rare-path counters
     double *bulk_rep;                        // [bulk_reps][rep_stride] replicas {J(S) | nu_bar(S) | luminosity sums(4) | ff_heating(S, continuum)}
     int bulk_reps;                           // power of two
@@ -563,47 +572,42 @@ template <bool FR> __device__ __forceinline__ void line_emission(Lane &p, int em
     if (FR) p.mu = aberration_cmf_to_lf(p.r, P.t_exp, p.mu);
 }
 
-// macro_atom.py:52-104 + interaction_event_callers.py:31-91 (classic branch)
+// macro_atom.py:52-104 + interaction_event_callers.py:31-91 (classic branch).  `entry`: P.macro_entry of the absorbed line.
 template <bool FR>
-__device__ __noinline__ void macro_atom_event(Lane &p, Rng &rng, int level,
+__device__ __noinline__ void macro_atom_event(Lane &p, Rng &rng, int2 entry,
                                                  unsigned long long &n_jumps, unsigned long long &n_scanned) {
     const KParams &P = cP;
-    int ttype = 0, tid = 0;
     // P.tp_t holds, per shell, the running sum of the transition probabilities inside each block, accumulated in
     // the reference's order (macro_cumsum_kernel): cum[tid] is bit-for-bit the `probability` the reference compares
     // with its random number after adding transition tid, so the first tid with cum[tid] > xi is found by bisection.
     const double *cum = P.tp_t + (size_t)p.shell * P.tpad;
-    while (ttype >= 0) {
+    const int *guide = P.macro_guide + (size_t)p.shell * P.tpad;
+    int2 next = entry;  // the block this jump draws from, or what ends the walk
+    while (next.x >= 0 || next.x == MNEXT_BAD_LEVEL) {
         double xi = rng.next_double();
         n_jumps++;
-        if (level < 0 || level >= P.n_blocks) { atomicMax(P.error, ERR_MACRO_ATOM); return; }
-        const int block_start = P.block_edge[level], block_end = P.block_edge[level + 1];
+        if (next.x < 0) { atomicMax(P.error, ERR_MACRO_ATOM); return; }  // a level outside the table
+        const int block_start = next.x, block_end = next.y;
         if (block_end <= block_start || !(cum[block_end - 1] > xi)) {  // "MacroAtom ran out of the block"
             n_scanned += (unsigned long long)(block_end - block_start);
             atomicMax(P.error, ERR_MACRO_ATOM);
             return;
         }
-        int lo = block_start, hi = block_end - 1;  // cum[hi] > xi
-        if (P.macro_guide) {
-            // bracket from the guide table: the answer lies between the entries of buckets k-1 and k+2 (one bucket of
-            // slack on each side covers the rounding of xi * n); cum is non-decreasing, so bisection inside is exact
-            const int *g = P.macro_guide + (size_t)p.shell * P.tpad + block_start;
-            const int n = block_end - block_start;
-            int k = (int)(xi * (double)n);
-            k = k < 0 ? 0 : (k > n - 1 ? n - 1 : k);
-            lo = g[k > 0 ? k - 1 : 0];
-            if (k + 2 < n) hi = g[k + 2];
-        }
+        // bracket from the guide table: the answer lies between the entries of buckets k-1 and k+2 (one bucket of
+        // slack on each side covers the rounding of xi * n); cum is non-decreasing, so bisection inside is exact
+        const int n = block_end - block_start;
+        int k = (int)(xi * (double)n);
+        k = k < 0 ? 0 : (k > n - 1 ? n - 1 : k);
+        int lo = guide[block_start + (k > 0 ? k - 1 : 0)];
+        int hi = (k + 2 < n) ? guide[block_start + k + 2] : block_end - 1;
         while (lo < hi) {
             const int mid = (lo + hi) >> 1;
             if (cum[mid] > xi) hi = mid; else lo = mid + 1;
         }
-        tid = lo;
-        n_scanned += (unsigned long long)(tid - block_start + 1);
-        level = P.dest[tid];
-        ttype = P.ttype[tid];
+        n_scanned += (unsigned long long)(lo - block_start + 1);
+        next = P.macro_next[lo];
     }
-    if (ttype == -1) line_emission<FR>(p, P.tline[tid]);
+    if (next.x == MNEXT_EMIT) line_emission<FR>(p, next.y);
     else atomicMax(P.error, ERR_MACRO_ATOM);
 }
 
@@ -1368,7 +1372,7 @@ __device__ __noinline__ void interaction_event_impl(Lane &p, Rng &rng, int itype
             double cnu = p.nu * old_dop;
             p.nu = cnu * inv_new;
             if (CONT) macro_atom_event_iip(p, rng, P.line2macro[p.next_line], c.jumps, c.scanned);
-            else macro_atom_event<FR>(p, rng, P.line2macro[p.next_line], c.jumps, c.scanned);
+            else macro_atom_event<FR>(p, rng, P.macro_entry[p.next_line], c.jumps, c.scanned);
         }
         log_interaction_after(p, IT_LINE);
         c.line_ev++;
@@ -2484,6 +2488,21 @@ __global__ void macro_guide_kernel(const double *tp_t, const int *block_edge, in
         while (tid < b1 - 1 && !(cum[tid] > thr)) tid++;
         g[b0 + k] = tid;
     }
+}
+
+// macro_next / macro_entry (see MNEXT_EMIT): one thread per transition, then one per line
+__device__ __forceinline__ int2 macro_block_of(int level, const int *block_edge, int n_blocks) {
+    return (level < 0 || level >= n_blocks) ? make_int2(MNEXT_BAD_LEVEL, 0) : make_int2(block_edge[level], block_edge[level + 1]);
+}
+__global__ void macro_next_kernel(const int *block_edge, const int *ttype, const int *dest, const int *tline, const int *line2macro,
+                                  int n_blocks, int n_transitions, int n_lines, int2 *next, int2 *entry) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_transitions) {
+        const int type = ttype[i];
+        next[i] = type >= 0 ? macro_block_of(dest[i], block_edge, n_blocks)
+                            : (type == -1 ? make_int2(MNEXT_EMIT, tline[i]) : make_int2(MNEXT_BAD_TYPE, 0));
+    }
+    if (i < n_lines) entry[i] = macro_block_of(line2macro[i], block_edge, n_blocks);
 }
 
 // IIP macro atom: running sums of the absorbing-Markov-chain probabilities along the destination axis, in the
