@@ -1205,7 +1205,7 @@ int tb200_line_accumulators(tb200_engine *en, void **device_ptr, int64_t *n_word
     if (en->algorithm != 1 || !en->diff.p) return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump)");
     *device_ptr = en->diff.p;
     *n_words = (int64_t)en->S * (en->lpad + 1) * 4;
-    *scale_j_blue = en->diff_scale1; *scale_edotlu = en->diff_scale2;
+    *scale_j_blue = en->diff_scale2; *scale_edotlu = en->diff_scale1;  // scale1: w1 -> Edotlu, scale2: w2 -> J_blue
     return TB200_OK;
 }
 

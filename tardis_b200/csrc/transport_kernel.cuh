@@ -381,10 +381,10 @@ __device__ __forceinline__ void red_u64(unsigned long long *addr, unsigned long 
 
 // word0 += floor(t / 2^29), word1 += round(t mod 2^29), with the typical term scaled to 2^58 (engine.cu).  Integer adds are
 // exact and order-independent, so the sums are bit-reproducible and cells that no packet touched stay exactly zero.
-// Headroom: a cell's low word holds 2^34 same-sign terms, its high word 2^34 typical ones (2^28 of the heaviest a line list
-// spanning a factor 40 in frequency can produce) before the signed reading in finalize_line_estimators_kernel would be off
-// by 2^64 -- and that kernel notices: every trace adds +w at its first line and -w behind its last, so each row must sum to
-// exactly zero (ERR_FIXED_POINT otherwise).
+// Headroom: a cell's low word holds 2^34 same-sign terms, its high word 2^33 typical ones (2^27 of the heaviest that equal
+// energies and a line list spanning a factor 40 in frequency can produce) before the signed reading in
+// finalize_line_estimators_kernel would be off by 2^64 -- and that kernel notices: every trace adds +w at its first line and
+// -w behind its last, so each row must sum to exactly zero and no prefix is negative (ERR_FIXED_POINT otherwise).
 // fixed_term converts w once (false, with ERR_FIXED_POINT raised, when w * scale is out of range); fixed_add adds it or its
 // negative to one cell.
 constexpr double FIXED_SPLIT = 536870912.0;  // 2^29
@@ -2592,6 +2592,7 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_line_estimators_kernel(c
     const double inv_scale = q == 0 ? inv_scale1 : inv_scale2;
     __shared__ unsigned long long tot_lo[32], tot_hi[32];  // inclusive scan of the warp totals of the current tile
     __int128 carry = 0;
+    bool negative = false;  // a finished prefix below zero (see the end of the kernel)
     for (int base = 0; base < lpad; base += FIN_THREADS) {
         const int i = base + threadIdx.x;
         __int128 x = 0;
@@ -2619,6 +2620,7 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_line_estimators_kernel(c
         if (warp > 0) x += (__int128)(((unsigned __int128)tot_hi[warp - 1] << 64) | tot_lo[warp - 1]);
         x += carry;
         if (i < n_lines) {
+            negative |= x < 0;
             double v = i128_to_double(x) * inv_scale;
             out[i] = full_rel ? v : v * nu_line[i];
         } else if (i < lpad) {
@@ -2628,9 +2630,13 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_line_estimators_kernel(c
         __syncthreads();  // the totals are overwritten by the next tile
     }
     // every range update is a +w / -w pair inside this row: a non-zero total means a 64-bit word wrapped (fixed_add).
+    // The total alone misses a wrap that the closing cell mirrors: a true sum of 2^63 + k at a range's first cell reads as
+    // -2^63 + k, the -2^63 - k behind its last line as 2^63 - k, and the row still sums to zero (sums over the members of
+    // a collective can get there).  But a prefix is a sum of the non-negative weights of the traces that cover the line,
+    // so a finished prefix below zero is a wrapped word too.
     // Unless an error already stopped the launch: the packets it was carrying keep the ranges that transfers opened
-    // (trace_range_end) unclosed, so the totals say nothing and the error that stopped it is the one to report.
-    if (threadIdx.x == 0 && carry != 0) atomicCAS(error, 0, ERR_FIXED_POINT);
+    // (trace_range_end) unclosed, so the sums say nothing and the error that stopped it is the one to report.
+    if (negative || (threadIdx.x == 0 && carry != 0)) atomicCAS(error, 0, ERR_FIXED_POINT);
 }
 
 // diff[s] += xfer[s - 1] - xfer[s] element-wise mod 2^64 (the transfers of trace_range_end; xfer has rows 0 .. S - 2).
