@@ -155,6 +155,11 @@ struct HostBins {
     std::vector<int> guide;    // [n_gkeys + 1]
     long long gkey_min = 0;
     int n_gkeys = 0;
+    // the continua active in bin g, in continuum order: act[2 i] = continuum k, act[2 i + 1] = phot_nus index of the lower
+    // point of its interval, for i in [act_start[g], act_start[g + 1]).  For a frequency strictly inside the bin these are
+    // exactly the continua and intervals the reference's threshold test and searchsorted select.
+    std::vector<int> act_start;  // [n_phot + 2]
+    std::vector<int> act;
     bool usable = false;       // false: the tables do not have the structure the bins assume -> literal path for every trace
 };
 
@@ -185,6 +190,17 @@ inline HostBins build_bins(const double *phot_nus, int n_phot, const long long *
         while (r < n_phot && (f64_bits(h.B[r]) >> GUIDE_SHIFT) < kmin + j) r++;
         h.guide[j] = r;
     }
+    h.act_start.assign(n_phot + 2, 0);
+    for (int g = 0; g <= n_phot; g++) {
+        h.act_start[g] = (int)(h.act.size() / 2);
+        if (g < 1 || g >= n_phot) continue;
+        for (int k = 0; k < n_continua; k++) {  // bin_chi_linear's selection (the blocks ascend strictly)
+            const int start = (int)refs[k], n = (int)(refs[k + 1] - refs[k]);
+            const int idx = block_rank(h.pos.data(), start, n, g);
+            if (idx >= 1 && idx <= n - 1) { h.act.push_back(k); h.act.push_back(start + idx - 1); }
+        }
+    }
+    h.act_start[n_phot + 1] = (int)(h.act.size() / 2);
     h.usable = true;
     return h;
 }

@@ -117,7 +117,7 @@ struct tb200_engine {
     int cont_bins = 0, cb_n_gkeys = 0;
     long long cb_gkey_min = 0;
     DBuf<double> cb_B, cb_mom, cont_lit;
-    DBuf<int> cb_guide, cb_nact, cb_pos;
+    DBuf<int> cb_guide, cb_nact, cb_pos, cb_act_start, cb_act;
     DBuf<double2> cb_chi_lin;
     size_t off_ffheat = 0, off_cont = 0, off_spec = 0, off_lum = 0;  // packed estimator buffer: ff_heating(S) and 5 x (n_continua * S)
     // packed estimators: [J(S) | nubar(S) | vhist(G) | pad | jblue(S*lpad) | edotlu(S*lpad)]
@@ -215,6 +215,7 @@ void tb200_destroy(tb200_engine *en) {
     en->prefix.release(); en->first_le.release(); en->diff.release(); en->xfer.release(); en->bulk_rep.release(); en->cnt_rep.release(); en->macro_guide.release(); en->macro_next.release(); en->macro_entry.release(); en->tp_t.release(); en->grid.release(); en->staging.release();
     en->t_e.release(); en->bf_thr.release(); en->pi_min.release(); en->pi_max.release(); en->x_sect.release(); en->phot_nus.release();
     en->cb_B.release(); en->cb_mom.release(); en->cont_lit.release(); en->cb_guide.release(); en->cb_nact.release(); en->cb_pos.release(); en->cb_chi_lin.release();
+    en->cb_act_start.release(); en->cb_act.release();
     en->ff_factor.release(); en->chi_bf_t.release(); en->emiss_t.release(); en->markov_cum.release(); en->pi_refs.release(); en->pi_act.release();
     en->mk_p_t.release(); en->mk_q.release(); en->mk_r.release(); en->mk_c.release(); en->mk_keep.release();
     en->mk_type.release(); en->mk_dest.release(); en->mk_err.release();
@@ -451,11 +452,14 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
             if (hb.usable) {
                 en->cb_gkey_min = hb.gkey_min; en->cb_n_gkeys = hb.n_gkeys;
                 if ((r = en->cb_B.ensure(nb)) || (r = en->cb_guide.ensure(hb.guide.size())) || (r = en->cb_nact.ensure(nb)) ||
-                    (r = en->cb_chi_lin.ensure((size_t)S * nb)))
+                    (r = en->cb_chi_lin.ensure((size_t)S * nb)) || (r = en->cb_act_start.ensure(hb.act_start.size())) ||
+                    (r = en->cb_act.ensure(hb.act.size())))
                     return r;
                 CK(cudaMemcpyAsync(en->cb_B.p, hb.B.data(), hb.B.size() * sizeof(double), cudaMemcpyHostToDevice, en->stream));
                 CK(cudaMemcpyAsync(en->cb_pos.p, hb.pos.data(), hb.pos.size() * sizeof(int), cudaMemcpyHostToDevice, en->stream));
                 CK(cudaMemcpyAsync(en->cb_guide.p, hb.guide.data(), hb.guide.size() * sizeof(int), cudaMemcpyHostToDevice, en->stream));
+                CK(cudaMemcpyAsync(en->cb_act_start.p, hb.act_start.data(), hb.act_start.size() * sizeof(int), cudaMemcpyHostToDevice, en->stream));
+                if (!hb.act.empty()) CK(cudaMemcpyAsync(en->cb_act.p, hb.act.data(), hb.act.size() * sizeof(int), cudaMemcpyHostToDevice, en->stream));
                 const long long total = (long long)S * nb;
                 tb::continuum_lin_kernel<<<(unsigned)((total + 127) / 128), 128, 0, en->stream>>>(en->cb_B.p, en->n_phot, en->phot_nus.p, en->cb_pos.p,
                     en->pi_refs.p, en->n_continua, en->chi_bf_t.p, en->phot_pad, S, en->cb_chi_lin.p, en->cb_nact.p);
@@ -784,6 +788,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         P.ff_opac_const = pow(2 * M_PI / (3 * m_el * k_b), 0.5) * 4 * pow(e_esu, 6) / (3 * m_el * h_pl * tb::C_LIGHT);
         P.cont_bins = en->cont_bins; P.cb_n_gkeys = en->cb_n_gkeys; P.cb_gkey_min = en->cb_gkey_min;
         P.cb_B = en->cb_B.p; P.cb_guide = en->cb_guide.p; P.cb_nact = en->cb_nact.p; P.cb_chi_lin = en->cb_chi_lin.p;
+        P.cb_act_start = en->cb_act_start.p; P.cb_act = reinterpret_cast<const int2 *>(en->cb_act.p);
         P.cb_mom = en->cb_mom.p; P.cont_lit = en->cont_lit.p;
     }
     P.full_rel = (en->cfg.enable_full_relativity || en->continuum) ? 1 : 0; P.line_mode = en->cfg.line_interaction_type;

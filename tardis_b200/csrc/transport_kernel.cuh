@@ -83,6 +83,8 @@ struct KParams {
     long long cb_gkey_min;
     const double *cb_B;                      // [n_phot] ascending union of the phot_nus blocks
     const int *cb_guide, *cb_nact;           // [cb_n_gkeys + 1]; [n_phot + 1] active continua per bin
+    const int *cb_act_start;                 // [n_phot + 2]: bin g's {continuum, lower phot_nus index} pairs are
+    const int2 *cb_act;                      //   cb_act[cb_act_start[g] .. cb_act_start[g + 1]) (HostBins::act)
     const double2 *cb_chi_lin;               // [S][n_phot + 1] {chi_bf_tot at the bin's left edge, slope}
     double *cb_mom;                          // [S][n_phot + 1][8] moments (tbc::trace_moments)
     double *cont_lit;                        // [5][n_continua][S] {photo_ion, stim_recomb, bf_heating, stim_recomb_cooling, statistics}
@@ -800,11 +802,25 @@ __device__ __noinline__ void macro_atom_event_iip(Lane &p, Rng &rng, int level, 
     else atomicMax(P.error, ERR_MACRO_ATOM);
 }
 
+// One term of chi_bf_contributions on the bins path: entry {k, lo} of the trace's bin (HostBins::act), interpolated with
+// phot_interp's weights and operation order, so the value is chi_bf_literal's term for continuum k.
+__device__ __forceinline__ double bin_chi_term(int2 e, double nu, const double *chi_row) {
+    const KParams &P = cP;
+    const double lo = P.phot_nus[e.y], hi = P.phot_nus[e.y + 1];
+    return (chi_row[e.y + 1] * (nu - lo) + chi_row[e.y] * (hi - nu)) / (hi - lo);
+}
+
 // continuum_event + determine_continuum_macro_activation_idx + determine_bf_macro_activation_idx
 // `trace_nu` is the comoving frequency at the START of the trace: the reference draws the absorbing continuum from the
 // chi_bf_contributions it computed there (modes/iip/packet_propagation.py:118-128,231-240), while the ionisation
-// fraction uses the comoving frequency at the interaction point.
-__device__ __noinline__ void continuum_event_impl(Lane &p, Rng &rng, double trace_nu, double chi_bf_tot, double chi_ff, Counters &c) {
+// fraction uses the comoving frequency at the interaction point.  fraction_bf and the normalisation of the draw use the
+// literal cumulative sum at trace_nu in continuum order, the reference's chi_bf_contributions[-1].  The trace's bins
+// value C + D (nu - B[g-1]) can differ from it in the last bits, or by far more where chi_bf cancels inside a bin, and
+// a draw above sum / bins value would find no continuum.  The trace distance and escat_prob stay on the bins value
+// (DESIGN section 2).  `trace_g` is the trace's bin, or -1 when the trace took the literal path (breakpoint tie, tables
+// without the bins' structure): then the active continua are searched as chi_bf_literal does, else they are read from
+// the bin's list.
+__device__ __noinline__ void continuum_event_impl(Lane &p, Rng &rng, double trace_nu, int trace_g, double chi_ff, Counters &c) {
     const KParams &P = cP;
     if (P.last_type || P.events) log_interaction_before(p, IT_CONTINUUM_PROCESS);
     const double velocity = p.r / P.t_exp;
@@ -815,18 +831,37 @@ __device__ __noinline__ void continuum_event_impl(Lane &p, Rng &rng, double trac
     const double comov_nu = p.nu * old_dop;
     p.energy = comov_energy * inv_dop;
     int destination = P.k_packet_idx;
+    const double *chi_row = P.chi_bf_t + (size_t)p.shell * P.phot_pad;
+    const int2 *act = nullptr;
+    int n_list = 0;
+    double chi_bf_tot = 0.0;
+    if (trace_g >= 0) {
+        act = P.cb_act + P.cb_act_start[trace_g];
+        n_list = P.cb_act_start[trace_g + 1] - P.cb_act_start[trace_g];
+        for (int i = 0; i < n_list; i++) chi_bf_tot += bin_chi_term(act[i], trace_nu, chi_row);
+    } else {
+        int n_act;
+        chi_bf_tot = chi_bf_literal(trace_nu, p.shell, &n_act);
+    }
     const double fraction_bf = chi_bf_tot / (chi_bf_tot + chi_ff);
     if (rng.next_double<true>() < fraction_bf) {
         // np.searchsorted(chi_bf_contributions, z): first active continuum with cumsum_i / chi_bf_tot >= z
         const double z = rng.next_double<true>();
-        const double *chi_row = P.chi_bf_t + (size_t)p.shell * P.phot_pad;
         double running = 0.0;
         int active = -1;
-        for (int k = 0; k < P.n_continua; k++) {
-            if (trace_nu >= P.pi_min[k] && trace_nu <= P.pi_max[k]) {
-                const PhotInterp w = phot_interp(k, trace_nu);
-                running += (chi_row[w.hi] * w.high_weight + chi_row[w.lo] * w.low_weight) / w.interval;
-                if (!(running / chi_bf_tot < z)) { active = k; break; }
+        if (trace_g >= 0) {
+            for (int i = 0; i < n_list; i++) {
+                const int2 e = act[i];
+                running += bin_chi_term(e, trace_nu, chi_row);
+                if (!(running / chi_bf_tot < z)) { active = e.x; break; }
+            }
+        } else {
+            for (int k = 0; k < P.n_continua; k++) {
+                if (trace_nu >= P.pi_min[k] && trace_nu <= P.pi_max[k]) {
+                    const PhotInterp w = phot_interp(k, trace_nu);
+                    running += (chi_row[w.hi] * w.high_weight + chi_row[w.lo] * w.low_weight) / w.interval;
+                    if (!(running / chi_bf_tot < z)) { active = k; break; }
+                }
             }
         }
         if (active < 0) { atomicMax(P.error, ERR_CONTINUUM); return; }
@@ -840,9 +875,9 @@ __device__ __noinline__ void continuum_event_impl(Lane &p, Rng &rng, double trac
     log_interaction_after(p, IT_CONTINUUM_PROCESS);
     c.cont_ev++;
 }
-__device__ __forceinline__ void continuum_event(Lane &p, Rng &rng, double trace_nu, double chi_bf_tot, double chi_ff, Counters &c) {
+__device__ __forceinline__ void continuum_event(Lane &p, Rng &rng, double trace_nu, int trace_g, double chi_ff, Counters &c) {
     Lane lp = p; Rng lr = rng; Counters lc;
-    continuum_event_impl(lp, lr, trace_nu, chi_bf_tot, chi_ff, lc);
+    continuum_event_impl(lp, lr, trace_nu, trace_g, chi_ff, lc);
     p = lp; rng = lr; flush_rare(lc);
 }
 
@@ -1710,7 +1745,7 @@ __global__ void __launch_bounds__(256, MIN_CTAS) transport_scan_kernel() {
             if (CONT) trace_bf_estimators(p, t, distance, s_ffh, c.bf_upd);
             move_and_bulk<FR, true>(p, distance, s_J, s_nubar);
             if (itype == IT_BOUNDARY) boundary_event(p, t.delta_shell, c);
-            else if (CONT && itype == IT_CONTINUUM_PROCESS) continuum_event_impl(p, rng, t.comov_nu, t.chi_bf_tot, t.chi_ff, c);
+            else if (CONT && itype == IT_CONTINUUM_PROCESS) continuum_event_impl(p, rng, t.comov_nu, t.cg, t.chi_ff, c);
             else interaction_event_impl<FR, CONT>(p, rng, itype, c);  // (on the state itself: see WarpFeed::refill)
             if (p.status != ST_IN_PROCESS) { finish_packet(p, rng, c); has = false; }
         }
@@ -2050,8 +2085,8 @@ __device__ __forceinline__ void event_phase_b(Lane &p, Rng &rng, Counters &c, do
     // (ESC -- continuum kernel, and the classic one when virtual packets are on: the handlers work on the packet state
     // itself, which keeps it in local memory -- see WarpFeed::refill; those kernels are bound by instruction supply)
     else if (CONT && itype == IT_CONTINUUM_PROCESS) {
-        if (ESC) continuum_event_impl(p, rng, t.comov_nu, t.chi_bf_tot, t.chi_ff, c);
-        else continuum_event(p, rng, t.comov_nu, t.chi_bf_tot, t.chi_ff, c);
+        if (ESC) continuum_event_impl(p, rng, t.comov_nu, t.cg, t.chi_ff, c);
+        else continuum_event(p, rng, t.comov_nu, t.cg, t.chi_ff, c);
     }
     else if (ESC) interaction_event_impl<FR, CONT, false>(p, rng, itype, c);
     else interaction_event<FR, CONT, false>(p, rng, itype, c);
