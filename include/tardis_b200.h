@@ -84,6 +84,9 @@ typedef struct {
     int64_t n_activation, k_packet_idx;
     int64_t n_markov;                            /* absorbing_markov_probabilities is [S, n_markov, n_markov] */
     const double *absorbing_markov_probabilities;
+    /* NumbaRadial1DGeometry (model/geometry/radial1d.py:320-375): shell-edge velocities, cm / s.  Read only when
+     * config.nonhomologous; the engine computes velocity_gradient = (v_outer - v_inner) / (r_outer - r_inner) itself. */
+    const double *v_inner, *v_outer;             /* [S] */
 } tb200_model;
 
 /* Replaces MonteCarloConfiguration (transport/montecarlo/configuration/base.py:11-49)
@@ -104,6 +107,12 @@ typedef struct {
     /* window of Simulation.iterate's calculate_filtered_luminosity (simulation/base.py:455-466, spectrum/luminosity.py:5-29;
      * config supernova.luminosity_wavelength_start/end converted to Hz), strict on both sides.  0 / +inf = everything. */
     double luminosity_nu_start, luminosity_nu_end;
+    /* 1: the nonhomologous transport mode (transport/montecarlo/modes/nonhomologous/): piecewise-linear velocity law from
+     * model.v_inner / v_outer, line distances from the quartic of calculate_distance_line_nonhomologous, two-way line scan;
+     * time_explosion is not used (0 is accepted).  Refused with full relativity ("Full relativity not supported for
+     * non-homology."), with continuum processes and without v_inner / v_outer.  Runs its own kernel whatever the
+     * options "algorithm" / "pooled" say; tb200_line_accumulators is refused and engine groups sum in f64 (exact = 0). */
+    int32_t nonhomologous;
 } tb200_config;
 
 /* Replaces PacketCollection inputs (transport/montecarlo/packets/packet_collections.py:14-76). */
@@ -254,6 +263,10 @@ typedef struct {
     double t_radiative_estimator_constant, sigma_sb, c, h, k_b;
     const double *j, *nu_bar;                        /* [S], or NULL = resident estimators */
     const double *j_blue;                            /* [L,S] C-order (with j) */
+    /* [S] or NULL.  The nonhomologous mode's solver (modes/nonhomologous/mc_rad_field_solver.py:35-131): J_blue is normalised
+     * by (c / velocity_gradient) / ((4 pi t_sim) V) instead of c t_exp / (4 pi t_sim V), and there is no optical window.
+     * Required (and only accepted) when the model was set with config.nonhomologous = 1. */
+    const double *velocity_gradient;
 } tb200_radfield_params;
 int tb200_solve_radiation_field(tb200_engine *engine, const tb200_radfield_params *params, double *t_radiative /* [S] */,
                                 double *dilution_factor /* [S] */, double *j_blues /* [L,S] C-order, or NULL */);

@@ -64,6 +64,7 @@ class Model(C.Structure):
         ("ff_opacity_factor", _pd), ("emissivities", _pd), ("photo_ion_activation_idx", _pi),
         ("n_activation", C.c_int64), ("k_packet_idx", C.c_int64), ("n_markov", C.c_int64),
         ("absorbing_markov_probabilities", _pd),
+        ("v_inner", _pd), ("v_outer", _pd),
     ]
 
 
@@ -76,6 +77,7 @@ class Config(C.Structure):
         ("vpacket_spawn_start_frequency", C.c_double), ("vpacket_spawn_end_frequency", C.c_double),
         ("spectrum_frequency_grid", _pd), ("n_grid", C.c_int64),
         ("luminosity_nu_start", C.c_double), ("luminosity_nu_end", C.c_double),
+        ("nonhomologous", C.c_int32),
     ]
 
 
@@ -104,6 +106,7 @@ class RadfieldParams(C.Structure):
         ("detailed_optical_window", C.c_int32),
         ("t_radiative_estimator_constant", C.c_double), ("sigma_sb", C.c_double), ("c", C.c_double), ("h", C.c_double), ("k_b", C.c_double),
         ("j", _pd), ("nu_bar", _pd), ("j_blue", _pd),
+        ("velocity_gradient", _pd),
     ]
 
 

@@ -18,6 +18,7 @@
 #include "opacity_build.cuh"
 #include "formal_integral.cuh"
 #include "markov_build.cuh"
+#include "nonhomologous.cuh"
 
 namespace {
 
@@ -103,6 +104,9 @@ struct tb200_engine {
     double finalize_ms = 0.0;
     bool est_unreduced = false;     // a transport filled the estimators since the last engine-group collective
     DBuf<int> line2macro, block_edge, ttype, dest, tline;
+    // nonhomologous mode (nonhomologous.cuh): NumbaRadial1DGeometry's v_inner / v_outer / velocity_gradient [S]
+    int nonhomologous = 0;
+    DBuf<double> v_inner, v_outer, dvdr;
     // continuum (IIP mode)
     int continuum = 0, n_continua = 0, n_phot = 0, phot_pad = 0, n_activation = 0, n_markov = 0;
     long long k_packet_idx = -1;
@@ -135,6 +139,7 @@ struct tb200_engine {
     // radiation-field solve (radfield.cuh): resident results + scratch for host-supplied estimators
     DBuf<double> rf_shell;   // [5 S]: t_rad, w, norm, j, nu_bar (the last two only with host-supplied estimators)
     DBuf<double> rf_volume, rf_jblues_t, rf_in_t;  // [S]; [S][lpad] normalised J_blue (shell-major); [S][lpad] uploaded estimator
+    DBuf<double> rf_dvdr;                          // [S] the caller's velocity_gradient (nonhomologous mode)
     // opacity build (opacity_build.cuh)
     bool opacity_pending = false;   // tb200_set_model got no tau_sobolev / transition_probabilities: tb200_build_opacity must run first
     bool have_macro = false;        // macro-atom metadata uploaded (line_interaction_type != scatter or continuum)
@@ -335,6 +340,11 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     if (c->line_interaction_type < 0 || c->line_interaction_type > 2) return fail(TB200_ERR_INVALID, "line_interaction_type must be 0, 1 or 2");
     for (int64_t i = 1; i < m->n_lines; i++)
         if (m->line_list_nu[i] > m->line_list_nu[i - 1]) return fail(TB200_ERR_INVALID, "line_list_nu must be sorted in descending order");
+    if (c->nonhomologous) {  // modes/nonhomologous: partial relativity and lines + electron scattering only
+        if (c->enable_full_relativity) return fail(TB200_ERR_INVALID, "Full relativity not supported for non-homology.");
+        if (c->continuum_processes_enabled) return fail(TB200_ERR_INVALID, "continuum processes are not supported in the nonhomologous mode");
+        if (!m->v_inner || !m->v_outer) return fail(TB200_ERR_INVALID, "the nonhomologous mode needs the model's v_inner and v_outer");
+    }
     en->have_model = false;
     en->sf_valid = false;
     en->diff_scale1 = en->diff_scale2 = 0.0;  // the difference arrays are zeroed below
@@ -352,6 +362,17 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     CK(cudaMemcpyAsync(en->r_inner.p, m->r_inner, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->r_outer.p, m->r_outer, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->n_e.p, m->electron_density, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+    en->nonhomologous = c->nonhomologous ? 1 : 0;
+    if (en->nonhomologous) {
+        // NumbaRadial1DGeometry.__init__ (model/geometry/radial1d.py:342-357): velocity_gradient by the reference's expression
+        std::vector<double> g((size_t)S);
+        for (int s = 0; s < S; s++) g[s] = nh::velocity_gradient(m->r_inner[s], m->r_outer[s], m->v_inner[s], m->v_outer[s]);
+        if ((r = en->v_inner.ensure(S)) || (r = en->v_outer.ensure(S)) || (r = en->dvdr.ensure(S))) return r;
+        CK(cudaMemcpyAsync(en->v_inner.p, m->v_inner, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+        CK(cudaMemcpyAsync(en->v_outer.p, m->v_outer, S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+        CK(cudaMemcpyAsync(en->dvdr.p, g.data(), S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+        CK(cudaStreamSynchronize(en->stream));  // g goes out of scope
+    }
     CK(cudaMemsetAsync(en->nu_line.p, 0, (en->lpad + TABLE_SLACK) * sizeof(double), en->stream));
     CK(cudaMemcpyAsync(en->nu_line.p, m->line_list_nu, L * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     en->opacity_pending = false;
@@ -723,8 +744,11 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
     CK(cudaSetDevice(en->device));
     const int S = en->S;
     const size_t row_words = (size_t)(en->lpad + 1) * 4;  // one shell's row of the difference arrays
+    // the nonhomologous kernel accumulates J_blue / Edotlu straight into the estimator buffer, as the scan kernel does:
+    // none of the jump algorithm's difference arrays, fixed-point scales or finalisation
+    const bool jump = en->algorithm == 1 && !en->nonhomologous;
     if (first) {
-        if (en->algorithm == 1) {  // the transfers of one call start from zero whatever happens to diff
+        if (jump) {  // the transfers of one call start from zero whatever happens to diff
             const size_t xfer_words = (size_t)(S > 1 ? S - 1 : 1) * row_words;
             int rx = en->xfer.ensure(xfer_words);
             if (rx) return rx;
@@ -732,7 +756,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         }
         if (zero_estimators) {
             CK(cudaMemsetAsync(en->est.p, 0, en->est_count * sizeof(double), en->stream));
-            if (en->algorithm == 1) CK(cudaMemsetAsync(en->diff.p, 0, (size_t)S * row_words * sizeof(unsigned long long), en->stream));
+            if (jump) CK(cudaMemsetAsync(en->diff.p, 0, (size_t)S * row_words * sizeof(unsigned long long), en->stream));
             if (en->continuum) {
                 CK(cudaMemsetAsync(en->cb_mom.p, 0, (size_t)S * (en->n_phot + 1) * tbc::N_MOMENTS * sizeof(double), en->stream));
                 CK(cudaMemsetAsync(en->cont_lit.p, 0, (size_t)5 * (en->n_continua > 0 ? en->n_continua : 1) * S * sizeof(double), en->stream));
@@ -747,15 +771,16 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
     }
     const int threads = en->threads_per_cta;
     const bool vpackets = !en->continuum && en->cfg.number_of_vpackets > 0;
-    const bool want_pool = en->algorithm == 1 && en->pooled && !vpackets;
-    const bool warp_volley = en->algorithm == 1 && vpackets;
+    const bool want_pool = jump && en->pooled && !vpackets;
+    const bool warp_volley = jump && vpackets;
     // resident CTAs per SM (x 256 threads), measured with scripts/perf_probe.py on the bench model on an H100 SXM at a 400 W power
     // limit: the pooled classic kernel (2e7 packets) is fastest at 2 of 1-4, the pooled continuum kernel (4e6 packets, 50 shells)
     // at 2 rather than 3, and the warp-volley kernel of virtual packets (1e8 packets x 10) at 2 rather than 3 (3.73 vs 3.90 s;
     // at 3 or 4 CTAs it is held to 80 / 64 registers and spills, at 2 it has 128 and none).  The lane-resident jump kernel
     // (option pooled = 0; 3 with continuum) and the scan kernel (3) are not re-measured on the H100.  Each kernel is compiled
     // for its own count (__launch_bounds__, the dispatch below); the option ctas_per_sm only sizes the grid, at most to what fits.
-    const int ctas_per_sm = en->ctas_per_sm > 0 ? en->ctas_per_sm : (en->algorithm == 1 ? (en->continuum ? (want_pool ? 2 : 3) : 2) : 3);
+    const int ctas_per_sm = en->ctas_per_sm > 0 ? en->ctas_per_sm
+                                                : (en->nonhomologous ? 2 : (en->algorithm == 1 ? (en->continuum ? (want_pool ? 2 : 3) : 2) : 3));
     const int grid = en->sm_count * ctas_per_sm;
     const size_t n_warps = (size_t)grid * (threads / 32);
     int r;
@@ -813,6 +838,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         P.macro_entry = (en->have_macro_guide && !en->continuum) ? en->macro_entry.p : nullptr;
         P.bulk_rep = en->bulk_rep.p; P.bulk_reps = BULK_REPS;
     }
+    if (en->nonhomologous) { P.v_inner = en->v_inner.p; P.v_outer = en->v_outer.p; P.dvdr = en->dvdr.p; }
     P.vol_min = en->vol_min;
     P.refill_min = en->refill_min > 0 ? en->refill_min : (pooled && !en->continuum ? 12 : 8); P.park_min = park_min; P.pool_slots = pool_slots; P.rng_units = rng_units;
     P.J = en->est.p + en->off_J; P.nubar = en->est.p + en->off_nubar; P.vhist = en->est.p + en->off_vhist;
@@ -829,7 +855,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         P.scale1 = ldexp(1.0, tb::FIXED_TYPICAL_LOG2 - ilogb(w1));
         P.scale2 = ldexp(1.0, tb::FIXED_TYPICAL_LOG2 - ilogb(w2));
         P.diff = en->diff.p; P.xfer = en->xfer.p;
-        if (en->algorithm == 1) {
+        if (jump) {
             // accumulating (zero_estimators == 0) into difference arrays that were filled at another scale would mix units
             if (first && zero_estimators) { en->diff_scale1 = 0.0; en->diff_scale2 = 0.0; }
             if (en->diff_scale1 != 0.0 && (en->diff_scale1 != P.scale1 || en->diff_scale2 != P.scale2))
@@ -872,11 +898,12 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
             P.vlog_nu = v; P.vlog_energy = v + cap; P.vlog_mu = v + 2 * cap; P.vlog_r = v + 3 * cap; P.vlog_pid = en->vlog_pid.p; P.vlog_capacity = cap;
         }
         size_t smem = (size_t)(en->algorithm == 1 ? 4 : 2) * S * sizeof(double);  // jump: [4 S] shell table; scan: J, nu_bar rows
+        if (en->nonhomologous) smem = 0;  // (its bulk estimators go to the global replicas)
         if (smem > 200 * 1024) return fail(TB200_ERR_INVALID, "too many shells for the shared-memory bulk estimators");
         if (pooled) {  // packet pools of the warps
             P.park_off = (int)(smem / sizeof(double));
             smem += (size_t)(threads / 32) * pool_slots * tb::pool_bytes_per_slot(en->continuum != 0);
-        } else if (en->algorithm == 1) {
+        } else if (jump) {
             // parked-lane columns (tb::TraceColumns), one per thread
             const bool cont = en->continuum != 0;
             P.park_off = (int)(smem / sizeof(double));
@@ -903,7 +930,9 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         CK(cudaMemcpyToSymbolAsync(tb::cP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, en->stream));
         if (ev_a) CK(cudaEventRecord(ev_a, en->stream));
         // one kernel per mode, compiled for the CTAs per SM its default runs at (see ctas_per_sm above)
-        if (en->continuum) {  // IIP mode: full relativity always (modes/iip/packet_propagation.py:104,123)
+        if (en->nonhomologous) {  // whatever the algorithm / pooled options say
+            TB_LAUNCH(nh::transport_nonhomologous_kernel);
+        } else if (en->continuum) {  // IIP mode: full relativity always (modes/iip/packet_propagation.py:104,123)
             if (pooled) TB_LAUNCH((tb::transport_pool_kernel<true, 2, true>));
             else if (en->algorithm == 1) TB_LAUNCH((tb::transport_jump_kernel<true, 3, true>));
             else TB_LAUNCH((tb::transport_scan_kernel<true, 2, true>));
@@ -937,7 +966,7 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
             CK(cudaGetLastError());
         }
     }
-    if (last && en->algorithm == 1) {
+    if (last && jump) {
         // diff[s] += xfer[s - 1] - xfer[s]: from here on diff holds every trace's +w / -w pair (trace_range_end)
         tb::fold_transfers_kernel<<<(unsigned)((row_words / 2 + 255) / 256), 256, 0, en->stream>>>(en->diff.p, en->xfer.p, S, row_words);
         en->launches++;
@@ -1207,7 +1236,8 @@ int tb200_run_resident(tb200_engine *en, tb200_outputs *o) {
 int tb200_line_accumulators(tb200_engine *en, void **device_ptr, int64_t *n_words, double *scale_j_blue, double *scale_edotlu) {
     if (!en || !device_ptr || !n_words || !scale_j_blue || !scale_edotlu) return fail(TB200_ERR_INVALID, "bad argument");
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
-    if (en->algorithm != 1 || !en->diff.p) return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump)");
+    if (en->algorithm != 1 || en->nonhomologous || !en->diff.p)
+        return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump), outside the nonhomologous mode");
     *device_ptr = en->diff.p;
     *n_words = (int64_t)en->S * (en->lpad + 1) * 4;
     *scale_j_blue = en->diff_scale2; *scale_edotlu = en->diff_scale1;  // scale1: w1 -> Edotlu, scale2: w2 -> J_blue
@@ -1217,7 +1247,8 @@ int tb200_line_accumulators(tb200_engine *en, void **device_ptr, int64_t *n_word
 int tb200_finalize_line_estimators(tb200_engine *en) {
     if (!en) return fail(TB200_ERR_INVALID, "bad argument");
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
-    if (en->algorithm != 1 || !en->diff.p) return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump)");
+    if (en->algorithm != 1 || en->nonhomologous || !en->diff.p)
+        return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump), outside the nonhomologous mode");
     if (en->diff_scale1 == 0.0 || en->diff_scale2 == 0.0) return fail(TB200_ERR_INVALID, "no transport has filled the line accumulators yet");
     CK(cudaSetDevice(en->device));
     const int full_rel = (en->cfg.enable_full_relativity || en->continuum) ? 1 : 0;
@@ -1238,13 +1269,17 @@ int tb200_estimator_buffer(tb200_engine *en, void **device_ptr, int64_t *n_doubl
 
 namespace {
 __global__ void radfield_shell_kernel(tbr::Constants K, const double *j, const double *nu_bar, const double *volume, double time_explosion,
-                                      double time_of_simulation, int n_shells, double *out /* [3 S]: t_rad, w, norm */) {
+                                      double time_of_simulation, int n_shells, double *out /* [3 S]: t_rad, w, norm */,
+                                      const double *dvdr /* [S] nonhomologous mode, or null */) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_shells) return;
     double t, w;
     tbr::dilute_planck(K, j[s], nu_bar[s], time_of_simulation, volume[s], &t, &w);
     out[s] = t; out[n_shells + s] = w;
-    out[2 * n_shells + s] = K.c * time_explosion / (4 * M_PI * time_of_simulation * volume[s]);  // j_blues_norm_factor
+    if (dvdr)  // modes/nonhomologous/mc_rad_field_solver.py:120-124
+        out[2 * n_shells + s] = (K.c / dvdr[s]) / (4 * M_PI * time_of_simulation * volume[s]);
+    else
+        out[2 * n_shells + s] = K.c * time_explosion / (4 * M_PI * time_of_simulation * volume[s]);  // j_blues_norm_factor
 }
 __global__ void radfield_jblue_kernel(tbr::Constants K, const double *est_t, const double *nu_line, const double *shell, int n_lines, int lpad,
                                       int n_shells, double w_epsilon, int window, double *out_t) {
@@ -1260,6 +1295,13 @@ int tb200_solve_radiation_field(tb200_engine *en, const tb200_radfield_params *p
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if ((p->j == nullptr) != (p->nu_bar == nullptr) || (p->j == nullptr) != (p->j_blue == nullptr))
         return fail(TB200_ERR_INVALID, "j, nu_bar and j_blue must be given together (or all NULL for the resident estimators)");
+    // a nonhomologous model carries no usable time_explosion: its J_blue normalisation needs the velocity gradient
+    if (en->nonhomologous && !p->velocity_gradient)
+        return fail(TB200_ERR_INVALID, "the nonhomologous mode normalises J_blue by c / velocity_gradient: pass velocity_gradient");
+    if (!en->nonhomologous && p->velocity_gradient)
+        return fail(TB200_ERR_INVALID, "velocity_gradient is the nonhomologous mode's normalisation; this model is homologous");
+    if (p->velocity_gradient && p->detailed_optical_window)
+        return fail(TB200_ERR_INVALID, "the nonhomologous radiation-field solver has no optical window");
     CK(cudaSetDevice(en->device));
     const int S = en->S, L = en->L, lpad = en->lpad;
     int r;
@@ -1275,7 +1317,12 @@ int tb200_solve_radiation_field(tb200_engine *en, const tb200_radfield_params *p
     }
     tbr::Constants K;
     K.t_radiative_estimator_constant = p->t_radiative_estimator_constant; K.sigma_sb = p->sigma_sb; K.c = p->c; K.h = p->h; K.k_b = p->k_b;
-    radfield_shell_kernel<<<(S + 127) / 128, 128, 0, st>>>(K, d_j, d_nubar, en->rf_volume.p, p->time_explosion, p->time_of_simulation, S, en->rf_shell.p);
+    if (p->velocity_gradient) {
+        if ((r = en->rf_dvdr.ensure(S))) return r;
+        CK(cudaMemcpyAsync(en->rf_dvdr.p, p->velocity_gradient, S * sizeof(double), cudaMemcpyHostToDevice, st));
+    }
+    radfield_shell_kernel<<<(S + 127) / 128, 128, 0, st>>>(K, d_j, d_nubar, en->rf_volume.p, p->time_explosion, p->time_of_simulation, S, en->rf_shell.p,
+                                                           p->velocity_gradient ? en->rf_dvdr.p : nullptr);
     const long long total = (long long)S * lpad;
     radfield_jblue_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(K, d_est_t, en->nu_line.p, en->rf_shell.p, L, lpad, S, p->w_epsilon,
                                                                           p->detailed_optical_window, en->rf_jblues_t.p);

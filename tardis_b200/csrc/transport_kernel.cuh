@@ -135,6 +135,8 @@ struct KParams {
     // ---- optional virtual packet log ----
     double *vlog_nu, *vlog_energy, *vlog_mu, *vlog_r; long long *vlog_pid; long long vlog_capacity;
     unsigned long long *vlog_count;
+    // ---- nonhomologous mode (nonhomologous.cuh): NumbaRadial1DGeometry's per-shell velocities [S] ----
+    const double *v_inner, *v_outer, *dvdr;
 };
 
 // Launch parameters live in constant memory: every field is a warp-uniform broadcast read, and the
@@ -574,8 +576,14 @@ template <bool FR> __device__ __forceinline__ void line_emission(Lane &p, int em
     if (FR) p.mu = aberration_cmf_to_lf(p.r, P.t_exp, p.mu);
 }
 
+// line_emission of the homologous modes, as the emitter of macro_atom_event
+template <bool FR> struct HomologousEmission {
+    __device__ __forceinline__ void operator()(Lane &p, int emission_line_id) const { line_emission<FR>(p, emission_line_id); }
+};
+
 // macro_atom.py:52-104 + interaction_event_callers.py:31-91 (classic branch).  `entry`: P.macro_entry of the absorbed line.
-template <bool FR>
+// The walk does not depend on the velocity law; EMIT is the line_emission of the caller's mode (nonhomologous.cuh has its own).
+template <bool FR, typename EMIT = HomologousEmission<FR>>
 __device__ __noinline__ void macro_atom_event(Lane &p, Rng &rng, int2 entry,
                                                  unsigned long long &n_jumps, unsigned long long &n_scanned) {
     const KParams &P = cP;
@@ -609,7 +617,7 @@ __device__ __noinline__ void macro_atom_event(Lane &p, Rng &rng, int2 entry,
         n_scanned += (unsigned long long)(lo - block_start + 1);
         next = P.macro_next[lo];
     }
-    if (next.x == MNEXT_EMIT) line_emission<FR>(p, next.y);
+    if (next.x == MNEXT_EMIT) EMIT()(p, next.y);
     else atomicMax(P.error, ERR_MACRO_ATOM);
 }
 

@@ -112,12 +112,20 @@ class Engine:
                   disable_line_scattering=False, sigma_thomson=SIGMA_THOMSON, number_of_vpackets=0,
                   survival_probability=0.0, vpacket_tau_russian=10.0, vpacket_spawn_start_frequency=0.0,
                   vpacket_spawn_end_frequency=1e200, continuum=None, t_electrons=None, luminosity_nu_start=0.0,
-                  luminosity_nu_end=np.inf):
+                  luminosity_nu_end=np.inf, nonhomologous=False, v_inner=None, v_outer=None):
         """`continuum`: object with the IIP fields of OpacityStateNumbaIIP (bf_threshold_list_nu,
         photo_ion_nu_threshold_mins/maxs, photo_ion_block_references, chi_bf, x_sect, phot_nus, ff_opacity_factor,
         emissivities, photo_ion_activation_idx, k_packet_idx, absorbing_markov_probabilities) -> IIP mode.
         absorbing_markov_probabilities = None (or transition_probabilities = None) leaves the continuum macro atom pending
-        until `build_absorbing_markov`."""
+        until `build_absorbing_markov`.
+        `nonhomologous`: the reference's nonhomologous mode, with the piecewise-linear velocity law of the shell-edge
+        velocities `v_inner` / `v_outer` [cm / s]; time_explosion is not used there."""
+        if nonhomologous and enable_full_relativity:
+            raise NotImplementedError("Full relativity not supported for non-homology.")
+        if nonhomologous and continuum is not None:
+            raise ValueError("continuum processes are not supported in the nonhomologous mode")
+        if nonhomologous and (v_inner is None or v_outer is None):
+            raise ValueError("the nonhomologous mode needs v_inner and v_outer")
         keep = []
         m = capi.Model()
         r_inner, r_outer, n_e, nu = _f64(r_inner), _f64(r_outer), _f64(electron_density), _f64(line_list_nu)
@@ -174,7 +182,14 @@ class Engine:
                 if cf["absorbing_markov_probabilities"].ndim != 3:
                     raise ValueError("absorbing_markov_probabilities must be [n_shells, n, n]")
                 m.n_markov = cf["absorbing_markov_probabilities"].shape[1]
+        if v_inner is not None and v_outer is not None:
+            vi, vo = _f64(v_inner), _f64(v_outer)
+            if len(vi) != len(r_inner) or len(vo) != len(r_inner):
+                raise ValueError("v_inner / v_outer must have one entry per shell")
+            keep += [vi, vo]
+            m.v_inner, m.v_outer = _dptr(vi), _dptr(vo)
         c = capi.Config()
+        c.nonhomologous = int(bool(nonhomologous))
         c.continuum_processes_enabled = int(continuum is not None)
         c.enable_full_relativity = int(bool(enable_full_relativity))
         c.line_interaction_type = mode
@@ -206,7 +221,8 @@ class Engine:
             line2macro_level_upper=mac.line2macro_level_upper, macro_block_edge_index=mac.macro_block_edge_index,
             transition_type=mac.transition_type, destination_level_id=mac.destination_level_id,
             transition_line_id=mac.transition_line_id, spectrum_frequency_grid=model.spectrum_frequency_grid,
-            continuum=getattr(model, "continuum", None), t_electrons=model.t_electrons, **config)
+            continuum=getattr(model, "continuum", None), t_electrons=model.t_electrons, v_inner=model.v_inner,
+            v_outer=model.v_outer, **config)
 
     # ---- packets ----
     def _packets_struct(self, initial_radii, initial_nus, initial_mus, initial_energies, packet_seeds):
@@ -528,10 +544,11 @@ class Engine:
 
     # ---- estimator -> radiation field (SURVEY.md §8f rank 4) ----
     def solve_radiation_field(self, *, time_explosion, time_of_simulation, volume, w_epsilon=1e-10, detailed_optical_window=False,
-                              estimators=None, want_j_blues=True):
+                              estimators=None, want_j_blues=True, velocity_gradient=None):
         """`tb200_solve_radiation_field`: T_rad, W per shell and the normalised / zero-filled J_blue table
         (MCRadiationFieldPropertiesSolver.solve, mc_rad_field_solver.py:37-144) from the estimators resident in HBM after
-        the last transport, or from `estimators = (j, nu_bar, j_blue[L,S])` given on the host."""
+        the last transport, or from `estimators = (j, nu_bar, j_blue[L,S])` given on the host.  `velocity_gradient` [S]: the
+        nonhomologous mode's solver (modes/nonhomologous/mc_rad_field_solver.py:35-131), required for a nonhomologous model."""
         from scipy.special import zeta  # noqa: PLC0415  (the reference computes its constant with scipy's zeta, :27-29)
 
         L, S, _ = self._model_shape
@@ -546,6 +563,12 @@ class Engine:
         p.t_radiative_estimator_constant = float((np.pi**4 / (15 * 24 * zeta(5, 1))) * (h / k_b))
         p.sigma_sb, p.c, p.h, p.k_b = sigma_sb, c, h, k_b
         keep = [vol]
+        if velocity_gradient is not None:
+            g = _f64(velocity_gradient)
+            if g.shape != (S,):
+                raise ValueError(f"velocity_gradient must have one entry per shell ({S})")
+            keep.append(g)
+            p.velocity_gradient = _dptr(g)
         if estimators is not None:
             j, nu_bar, j_blue = (_f64(a) for a in estimators)
             if j.shape != (S,) or nu_bar.shape != (S,) or j_blue.shape != (L, S):

@@ -396,6 +396,9 @@ def montecarlo_transport_with_vpackets(
     eng = engine or get_engine()
     o = opacity_state_numba
     grid = np.ascontiguousarray(_value(spectrum_frequency_grid), dtype=np.float64)
+    # the geometry carrier decides the mode: NumbaRadial1DGeometry (model/geometry/radial1d.py:320-375) holds a per-shell
+    # velocity_gradient -> the nonhomologous mode; NumbaHomologousRadial1DGeometry holds the scalar 1 / t_exp
+    nonhomologous = np.ndim(getattr(geometry_state_numba, "velocity_gradient", 0.0)) == 1
     line_mode = int(cfg.LINE_INTERACTION_TYPE)
     if int(cfg.NUMBER_OF_VPACKETS) != int(number_of_vpackets):
         logger.debug("number_of_vpackets differs from configuration; using the argument, like the reference")
@@ -415,6 +418,9 @@ def montecarlo_transport_with_vpackets(
         vpacket_spawn_start_frequency=float(cfg.VPACKET_SPAWN_START_FREQUENCY),
         vpacket_spawn_end_frequency=float(cfg.VPACKET_SPAWN_END_FREQUENCY),
         luminosity_nu_start=float(_value(luminosity_nu_start)), luminosity_nu_end=float(_value(luminosity_nu_end)),
+        nonhomologous=nonhomologous,
+        v_inner=_value(geometry_state_numba.v_inner) if nonhomologous else None,
+        v_outer=_value(geometry_state_numba.v_outer) if nonhomologous else None,
     )
     pc = packet_collection
     n = len(pc.initial_nus)
@@ -948,3 +954,105 @@ class MCTransportSolverB200IIP(MCTransportSolverB200):
         transport_state.tracker_last_interaction_df = trackers.to_df()
         transport_state.virt_logging = False
         return np.zeros_like(np.asarray(_value(self.spectrum_frequency_grid), dtype=np.float64))
+
+
+# --------------------------------------------------------------------------------------
+# the nonhomologous mode (transport/montecarlo/modes/nonhomologous/)
+# --------------------------------------------------------------------------------------
+class MonteCarloTransportStateB200Nonhomologous(MonteCarloTransportState):
+    """modes/nonhomologous/montecarlo_transport_state.py:8-288: the classic state without time_explosion (same
+    properties)."""
+
+    def __init__(self, packet_collection, geometry_state_numba, opacity_state_numba, n_levels_bf_species_by_n_cells_tuple,
+                 tracker_full_df=None, tracker_last_interaction_df=None, vpacket_tracker=None):
+        super().__init__(packet_collection, geometry_state_numba, opacity_state_numba, None,
+                         n_levels_bf_species_by_n_cells_tuple=n_levels_bf_species_by_n_cells_tuple,
+                         tracker_full_df=tracker_full_df, tracker_last_interaction_df=tracker_last_interaction_df,
+                         vpacket_tracker=vpacket_tracker)
+
+
+class MCRadiationFieldPropertiesSolverB200Nonhomologous(MCRadiationFieldPropertiesSolverB200):
+    """Drop-in for the nonhomologous ``MCRadiationFieldPropertiesSolver`` (modes/nonhomologous/mc_rad_field_solver.py:35-131):
+    J_blue normalised by (c / velocity_gradient) / (4 pi t_sim V), no optical window."""
+
+    def solve(self, estimators_bulk, estimators_line, velocity_gradient, time_of_simulation, volume, line_list_nu):
+        eng = get_engine(self.device)
+        last = getattr(montecarlo_transport_with_vpackets, "last_estimators", None)
+        resident = (last is not None and last[0] is eng and estimators_bulk.mean_intensity_total is last[1]
+                    and estimators_bulk.mean_frequency is last[2] and estimators_line.mean_intensity_blueward is last[3])
+        est = None if resident else (estimators_bulk.mean_intensity_total, estimators_bulk.mean_frequency,
+                                     estimators_line.mean_intensity_blueward)
+        t_rad, w, j_blues = eng.solve_radiation_field(time_explosion=0.0, time_of_simulation=float(_value(time_of_simulation)),
+                                                      volume=_value(volume), w_epsilon=self.w_epsilon, estimators=est,
+                                                      velocity_gradient=_value(velocity_gradient))
+        return EstimatedRadiationFieldProperties(DilutePlanckianRadiationField(_quantity(t_rad, "K"), w), j_blues)
+
+
+class MCTransportSolverB200Nonhomologous(MCTransportSolverB200):
+    """Drop-in for ``MCTransportSolverNonhomologous`` (modes/nonhomologous/solver.py:48-358): the geometry carrier is
+    NumbaRadial1DGeometry, the loop runs with time_explosion = 0.0, partial relativity only."""
+
+    def initialize_transport_state(self, simulation_state, opacity_state, macro_atom_state, plasma, no_of_packets,
+                                   no_of_virtual_packets=0, iteration=0):
+        """modes/nonhomologous/solver.py:101-147 (opacities sliced by the r boundary indices)"""
+        species = getattr(plasma, "continuum_interaction_species", None)
+        if species is not None and not getattr(species, "empty", True):
+            gamma = getattr(plasma, "gamma", None)
+            n_levels_bf_species_by_n_cells_tuple = gamma.shape if gamma is not None else plasma.phi_lucy.shape
+        else:
+            n_levels_bf_species_by_n_cells_tuple = (0, 0)
+        packet_collection = self.packet_source.create_packets(no_of_packets, seed_offset=iteration)
+        geometry_state = simulation_state.geometry.to_numba()
+        opacity_state_numba = opacity_state.to_numba(macro_atom_state, self.line_interaction_type)
+        geo = simulation_state.geometry
+        opacity_state_numba = opacity_state_numba[geo.r_inner_boundary_index: geo.r_outer_boundary_index]
+        transport_state = MonteCarloTransportStateB200Nonhomologous(
+            packet_collection, geometry_state_numba=geometry_state, opacity_state_numba=opacity_state_numba,
+            n_levels_bf_species_by_n_cells_tuple=n_levels_bf_species_by_n_cells_tuple)
+        transport_state.enable_full_relativity = self.montecarlo_configuration.ENABLE_FULL_RELATIVITY
+        configuration_initialize(self.montecarlo_configuration, self, no_of_virtual_packets)
+        return transport_state
+
+    def run(self, transport_state, show_progress_bars=True):
+        """modes/nonhomologous/solver.py:149-268: returns ``v_packets_energy_hist``; the estimators, the last-interaction
+        DataFrame and (with virtual-packet logging) the vpacket tracker go on the state."""
+        if self.montecarlo_configuration.ENABLE_FULL_RELATIVITY:
+            raise NotImplementedError("Full relativity not supported for non-homology.")
+        self.transport_state = transport_state
+        cfg = self.montecarlo_configuration
+        number_of_vpackets = cfg.NUMBER_OF_VPACKETS
+        trackers = generate_tracker_last_interaction_list(len(transport_state.packet_collection.initial_nus))
+        v_packets_energy_hist, vpacket_tracker, estimators_bulk, estimators_line = montecarlo_transport_with_vpackets(
+            transport_state.packet_collection, transport_state.geometry_state_numba, 0.0,
+            transport_state.opacity_state_numba, cfg, _value(self.spectrum_frequency_grid), trackers,
+            number_of_vpackets, show_progress_bars=show_progress_bars, packet_propagation_function=None,
+            engine=get_engine(self.device), sigma_thomson=self.sigma_thomson,
+            luminosity_nu_start=self.luminosity_nu_start, luminosity_nu_end=self.luminosity_nu_end)
+        transport_state.fused_packet_sums = montecarlo_transport_with_vpackets.last_fused
+        transport_state.estimators_bulk = estimators_bulk
+        transport_state.estimators_line = estimators_line
+        if cfg.ENABLE_VPACKET_TRACKING and number_of_vpackets > 0:
+            transport_state.vpacket_tracker = vpacket_tracker
+        transport_state.tracker_full_df = None
+        transport_state.tracker_last_interaction_df = trackers.to_df()
+        transport_state.virt_logging = cfg.ENABLE_VPACKET_TRACKING
+        return v_packets_energy_hist
+
+    run_nonhomologous = run
+
+    @classmethod
+    def from_config(cls, config, packet_source, enable_virtual_packet_logging=False, device=0,
+                    honor_disable_electron_scattering=False):
+        """modes/nonhomologous/solver.py:271-358 (as MCTransportSolverB200.from_config, with the nonhomologous
+        radiation-field solver)."""
+        solver = super().from_config(config, packet_source, enable_virtual_packet_logging=enable_virtual_packet_logging,
+                                     device=device, honor_disable_electron_scattering=honor_disable_electron_scattering)
+        try:
+            from tardis.transport.montecarlo.modes.nonhomologous.mc_rad_field_solver import (  # noqa: PLC0415
+                MCRadiationFieldPropertiesSolver,
+            )
+
+            solver.radfield_prop_solver = MCRadiationFieldPropertiesSolver(config.plasma.w_epsilon)
+        except Exception:  # not importable: the engine's own (same surface)
+            solver.radfield_prop_solver = MCRadiationFieldPropertiesSolverB200Nonhomologous(config.plasma.w_epsilon, device=device)
+        return solver

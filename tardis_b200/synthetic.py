@@ -557,3 +557,20 @@ def make_plasma_state(atomic: AtomicData, n_shells: int, time_explosion: float, 
     L = len(atomic.nu)
     j_blues = 10 ** rng.uniform(-9, -5, (L, n_shells))
     return PlasmaState(np.ascontiguousarray(lnd), np.ascontiguousarray(j_blues), float(time_explosion))
+
+
+def make_nonhomologous_velocities(model: Model, amplitude: float = 0.08, seed: int = MODEL_SEED + 9) -> Model:
+    """A copy of `model` for the nonhomologous mode: radii kept, the interior shell-edge velocities multiplied by
+    1 + amplitude * U(-1, 1) (deterministic in `seed`).  The innermost and outermost edges are kept.  If no shell ends up
+    decelerating (v_outer < v_inner), the middle interior edge is raised above its outer neighbour, so at least one
+    shell scans its lines backwards."""
+    import dataclasses
+
+    v = np.concatenate([model.v_inner, model.v_outer[-1:]]).astype(np.float64)
+    rng = np.random.default_rng(seed)
+    if len(v) > 2:
+        v[1:-1] *= 1.0 + amplitude * rng.uniform(-1.0, 1.0, len(v) - 2)
+        if not np.any(v[1:] < v[:-1]):
+            k = (len(v) - 1) // 2
+            v[k] = v[k + 1] * (1.0 + 0.5 * amplitude)
+    return dataclasses.replace(model, v_inner=np.ascontiguousarray(v[:-1]), v_outer=np.ascontiguousarray(v[1:]))
