@@ -347,9 +347,14 @@ typedef struct {
 } tb200_atomic_data;
 typedef struct {
     const double *level_number_density;      /* [n_levels, S] C-order */
-    double time_explosion;                   /* s */
+    double time_explosion;                   /* s (not read in the nonhomologous mode) */
     const double *j_blues;                   /* [L,S] C-order, or NULL = the table tb200_solve_radiation_field left in HBM
                                                 (only read by the macro atom's internal-up rows) */
+    /* Nonhomologous mode (config.nonhomologous): required, and refused on a homologous model.  The active shells'
+     * dv/dr; tau = lambda f_lu COEFF / velocity_gradient * stim * n_lower (modes/nonhomologous/tau_sobolev.py:55-61)
+     * instead of ... * time_explosion * ...  A shell with velocity_gradient < 0 has tau < 0 (and beta > 1), as in the
+     * reference; velocity_gradient == 0 is the reference's "Some tau_sobolevs are nan, inf, -inf" error. */
+    const double *velocity_gradient;         /* [S], 1/s */
 } tb200_plasma_state;
 int tb200_set_atomic_data(tb200_engine *engine, const tb200_atomic_data *atomic);
 int tb200_build_opacity(tb200_engine *engine, const tb200_plasma_state *plasma);

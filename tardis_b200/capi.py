@@ -125,7 +125,7 @@ class AtomicData(C.Structure):
 
 class PlasmaState(C.Structure):
     """tb200_plasma_state"""
-    _fields_ = [("level_number_density", _pd), ("time_explosion", C.c_double), ("j_blues", _pd)]
+    _fields_ = [("level_number_density", _pd), ("time_explosion", C.c_double), ("j_blues", _pd), ("velocity_gradient", _pd)]
 
 
 class MarkovInput(C.Structure):

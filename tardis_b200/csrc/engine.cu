@@ -160,6 +160,7 @@ struct tb200_engine {
     DBuf<int> at_lower, at_upper;
     DBuf<unsigned char> at_meta, at_nlte;
     DBuf<double> at_g, at_wfl, at_flu, at_ful, at_elo, at_eup, op_lnd, op_beta_t, op_stim_t, op_tp_norm_t;
+    DBuf<double> op_dvdr;  // [S] the caller's velocity_gradient of tb200_build_opacity (nonhomologous mode)
     // control
     DBuf<unsigned> rng_buf;
     DBuf<unsigned long long> ctrl;  // [0] next_packet, [1] vlog_count, [2..] counters
@@ -230,7 +231,7 @@ void tb200_destroy(tb200_engine *en) {
     en->order.release(); en->order_hist.release();
     en->at_lower.release(); en->at_upper.release(); en->at_meta.release(); en->at_nlte.release(); en->at_g.release(); en->at_wfl.release();
     en->at_flu.release(); en->at_ful.release(); en->at_elo.release(); en->at_eup.release(); en->op_lnd.release(); en->op_beta_t.release();
-    en->op_stim_t.release(); en->op_tp_norm_t.release();
+    en->op_stim_t.release(); en->op_tp_norm_t.release(); en->op_dvdr.release();
     en->sf_lvl_ptr.release(); en->sf_lvl_lines.release(); en->sf_in_ptr.release(); en->sf_in_rows.release(); en->sf_in_src.release(); en->sf_em_row.release();
     en->fi_cells.release(); en->fi_shells.release(); en->fi_weights.release(); en->fi_freq.release(); en->fi_I.release(); en->fi_L.release();
     en->fi_att_t.release(); en->fi_jred_t.release(); en->fi_jblue_t.release();
@@ -1695,9 +1696,19 @@ int tb200_formal_integral_ms(tb200_engine *en, double *interpolation_ms, double 
 
 // ---- opacity build (opacity_build.cuh) ----------------------------------------------------------------------------------
 namespace {
-__global__ void opacity_line_kernel(tbo::Constants K, const double *lnd, int n_shells, const int *lower, const int *upper, const double *g,
-                                    const unsigned char *meta, const unsigned char *nlte, const double *wfl, double time_explosion, int n_lines,
-                                    int lpad, double *tau_t, double *beta_t, double *stim_t, int *error) {
+// The mode's tau formula, chosen at compile time by the type of `scale`: the homologous mode's time_explosion, or the
+// nonhomologous mode's velocity_gradient [S] (the caller's array).  One body, one kernel per mode.
+extern "C++" {
+__device__ __forceinline__ double line_tau(const tbo::Constants &K, double wfl, double time_explosion, int, double stim, double n_lower) {
+    return tbo::tau_sobolev(K, wfl, time_explosion, stim, n_lower);
+}
+__device__ __forceinline__ double line_tau(const tbo::Constants &K, double wfl, const double *velocity_gradient, int s, double stim, double n_lower) {
+    return tbo::tau_sobolev_nonhomologous(K, wfl, velocity_gradient[s], stim, n_lower);
+}
+template <typename Scale>
+__device__ __forceinline__ void opacity_line_cells(const tbo::Constants &K, const double *lnd, int n_shells, const int *lower, const int *upper,
+                                                   const double *g, const unsigned char *meta, const unsigned char *nlte, const double *wfl,
+                                                   Scale scale, int n_lines, int lpad, double *tau_t, double *beta_t, double *stim_t, int *error) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long long)n_shells * lpad) return;
     const int s = (int)(i / lpad), l = (int)(i % lpad);
@@ -1706,11 +1717,23 @@ __global__ void opacity_line_kernel(tbo::Constants K, const double *lnd, int n_s
         const int lo = lower[l], up = upper[l];
         const double n_lower = lnd[(size_t)lo * n_shells + s], n_upper = lnd[(size_t)up * n_shells + s];
         stim = tbo::stimulated_emission_factor(n_lower, n_upper, g[lo], g[up], meta[up] != 0, nlte ? nlte[l] != 0 : false);
-        tau = tbo::tau_sobolev(K, wfl[l], time_explosion, stim, n_lower);
+        tau = line_tau(K, wfl[l], scale, s, stim, n_lower);
         if (isnan(tau) || isinf(tau)) atomicMax(error, tb::ERR_OPACITY);  // "Some tau_sobolevs are nan, inf, -inf" (tau_sobolev.py:63-67)
         beta = tbo::beta_sobolev(tau);
     }
     tau_t[i] = tau; beta_t[i] = beta; stim_t[i] = stim;
+}
+}  // extern "C++"
+__global__ void opacity_line_kernel(tbo::Constants K, const double *lnd, int n_shells, const int *lower, const int *upper, const double *g,
+                                    const unsigned char *meta, const unsigned char *nlte, const double *wfl, double time_explosion, int n_lines,
+                                    int lpad, double *tau_t, double *beta_t, double *stim_t, int *error) {
+    opacity_line_cells(K, lnd, n_shells, lower, upper, g, meta, nlte, wfl, time_explosion, n_lines, lpad, tau_t, beta_t, stim_t, error);
+}
+__global__ void opacity_line_nonhomologous_kernel(tbo::Constants K, const double *lnd, int n_shells, const int *lower, const int *upper,
+                                                  const double *g, const unsigned char *meta, const unsigned char *nlte, const double *wfl,
+                                                  const double *velocity_gradient, int n_lines, int lpad, double *tau_t, double *beta_t,
+                                                  double *stim_t, int *error) {
+    opacity_line_cells(K, lnd, n_shells, lower, upper, g, meta, nlte, wfl, velocity_gradient, n_lines, lpad, tau_t, beta_t, stim_t, error);
 }
 __global__ void opacity_row_kernel(tbo::Constants K, const int *ttype, const int *tline, const double *beta_t, const double *stim_t,
                                    const double *jblues_t, const double *nu, const double *f_ul, const double *f_lu, const double *e_lo,
@@ -1782,6 +1805,11 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
     const bool need_jblues = en->have_macro && en->cfg.line_interaction_type == 2;
     if (need_jblues && !p->j_blues && !en->rf_valid)
         return fail(TB200_ERR_INVALID, "j_blues is NULL and tb200_solve_radiation_field has not left a table in HBM");
+    // a nonhomologous model carries no usable time_explosion: its tau divides by the velocity gradient instead
+    if (en->nonhomologous && !p->velocity_gradient)
+        return fail(TB200_ERR_INVALID, "the nonhomologous mode's tau_sobolev divides by velocity_gradient: pass velocity_gradient");
+    if (!en->nonhomologous && p->velocity_gradient)
+        return fail(TB200_ERR_INVALID, "velocity_gradient is the nonhomologous mode's tau_sobolev; this model is homologous");
     CK(cudaSetDevice(en->device));
     const int S = en->S, L = en->L, lpad = en->lpad;
     int r;
@@ -1791,8 +1819,16 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
     CK(cudaMemsetAsync(en->error.p, 0, sizeof(int), st));
     {
         const long long total = (long long)S * lpad;
-        opacity_line_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(en->op_const, en->op_lnd.p, S, en->at_lower.p, en->at_upper.p, en->at_g.p,
-            en->at_meta.p, en->at_nlte.p, en->at_wfl.p, p->time_explosion, L, lpad, en->tau_t.p, en->op_beta_t.p, en->op_stim_t.p, en->error.p);
+        const unsigned grid = (unsigned)((total + 255) / 256);
+        if (en->nonhomologous) {
+            if ((r = en->op_dvdr.ensure(S))) return r;
+            CK(cudaMemcpyAsync(en->op_dvdr.p, p->velocity_gradient, S * sizeof(double), cudaMemcpyHostToDevice, st));
+            opacity_line_nonhomologous_kernel<<<grid, 256, 0, st>>>(en->op_const, en->op_lnd.p, S, en->at_lower.p, en->at_upper.p, en->at_g.p,
+                en->at_meta.p, en->at_nlte.p, en->at_wfl.p, en->op_dvdr.p, L, lpad, en->tau_t.p, en->op_beta_t.p, en->op_stim_t.p, en->error.p);
+        } else {
+            opacity_line_kernel<<<grid, 256, 0, st>>>(en->op_const, en->op_lnd.p, S, en->at_lower.p, en->at_upper.p, en->at_g.p, en->at_meta.p,
+                en->at_nlte.p, en->at_wfl.p, p->time_explosion, L, lpad, en->tau_t.p, en->op_beta_t.p, en->op_stim_t.p, en->error.p);
+        }
         en->launches++;
         CK(cudaGetLastError());
     }

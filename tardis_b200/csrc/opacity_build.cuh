@@ -4,6 +4,7 @@
 // What it replaces (paths relative to /root/reference/tardis/):
 //   StimulatedEmissionFactor.calculate                 plasma/properties/radiative_properties.py:66-116
 //   calculate_sobolev_line_opacity                     opacities/tau_sobolev.py:21-75
+//     (nonhomologous mode: divided by the velocity gradient)  transport/montecarlo/modes/nonhomologous/tau_sobolev.py:21-75
 //   numba_calculate_beta_sobolev                       opacities/tau_sobolev.py:77-88
 //   probability_emission_down / _internal_down / _internal_up   opacities/macro_atom/macroatom_line_transitions.py:94-139,213-247,324-367
 //   BoundBoundMacroAtomSolver.normalize_transition_probabilities / _solve_next_macroatom_iteration
@@ -43,6 +44,13 @@ TBO_HD double stimulated_emission_factor(double n_lower, double n_upper, double 
 // calculate_sobolev_line_opacity, one cell: ((((lambda f_lu) * COEFF) * t_exp) * stim) * n_lower
 TBO_HD double tau_sobolev(const Constants &K, double wavelength_f_lu, double time_explosion, double stim, double n_lower) {
     return wavelength_f_lu * K.sobolev_coefficient * time_explosion * stim * n_lower;
+}
+
+// the nonhomologous mode's calculate_sobolev_line_opacity (transport/montecarlo/modes/nonhomologous/tau_sobolev.py:21-75),
+// one cell: ((((lambda f_lu) * COEFF) / dvdr) * stim) * n_lower.  dvdr < 0 (a decelerating shell) gives tau < 0, as there;
+// dvdr == 0 gives +-inf or NaN, which the build reports as the reference's ValueError.
+TBO_HD double tau_sobolev_nonhomologous(const Constants &K, double wavelength_f_lu, double velocity_gradient, double stim, double n_lower) {
+    return wavelength_f_lu * K.sobolev_coefficient / velocity_gradient * stim * n_lower;
 }
 
 // numba_calculate_beta_sobolev, one cell

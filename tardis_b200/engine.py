@@ -402,9 +402,11 @@ class Engine:
         a.c, a.h = c, h
         self._check(self._api("set_atomic_data")(self._h, C.byref(a)))
 
-    def build_opacity(self, level_number_density, time_explosion, j_blues=None):
+    def build_opacity(self, level_number_density, time_explosion, j_blues=None, velocity_gradient=None):
         """`tb200_build_opacity`: tau_Sobolev, beta_Sobolev and the normalised macro-atom probabilities of this iteration, built
-        in HBM from the level populations [n_levels, S] (and J_blue: `None` = the table `solve_radiation_field` left resident)."""
+        in HBM from the level populations [n_levels, S] (and J_blue: `None` = the table `solve_radiation_field` left resident).
+        `velocity_gradient` [S] (1/s): the nonhomologous mode's tau (modes/nonhomologous/tau_sobolev.py:21-75), required for a
+        nonhomologous model, whose `time_explosion` is then not read."""
         p = capi.PlasmaState()
         lnd = _f64(level_number_density)
         keep = [lnd]
@@ -413,6 +415,13 @@ class Engine:
             jb = _f64(j_blues)
             keep.append(jb)
             p.j_blues = _dptr(jb)
+        if velocity_gradient is not None:
+            g = _f64(velocity_gradient)
+            S = self._model_shape[1]
+            if g.shape != (S,):
+                raise ValueError(f"velocity_gradient must have one entry per shell ({S})")
+            keep.append(g)
+            p.velocity_gradient = _dptr(g)
         self._check(self._api("build_opacity")(self._h, C.byref(p)))
 
     def download_opacity(self, transition_probabilities=False):
