@@ -333,6 +333,40 @@ int tb200_formal_integral_ms(tb200_engine *engine, double *interpolation_ms, dou
  * leaves the opacity tables pending; tb200_set_atomic_data once; then every iteration tb200_build_opacity fills the
  * tables in HBM (shell-major, with the prefix sums / running sums / guide tables the kernels read) from the level
  * populations and from J_blue -- the copy tb200_solve_radiation_field left resident, or a host array. */
+/* The continuum mode's static row map (given once, with the atomic data): for every macro-atom row, which row of which
+ * per-iteration table of tb200_continuum_rates it reads, and its energy factor, resolved on the host exactly as
+ * ContinuumMacroAtomSolver._solve_next_macroatom_iteration (opacities/macro_atom/macroatom_solver.py:1533-1631) looks them
+ * up: by label (.loc) for PHOTOIONIZATION_INTERNAL (2) / PHOTO_RECOMB_INTERNAL (3), by collision_key_idx (.iloc) for the
+ * collisional rows (11, 5, 4, 6, 7, 14), by position inside the type for PHOTO_RECOMB_EMISSION (-7) and the cooling rows
+ * (-20, 21, 22; normalize_cooling_block_by_rate_fractions, :1817-1833).  The map belongs to the model current when it is
+ * given: tb200_set_model discards it, and the continuum build refuses to run until tb200_set_atomic_data gives it again.  The table follows from the row's transition_type
+ * (the model's): 2 -> rate[0], 3 / -7 -> rate[1], 11 / 5 -> rate[2], 4 -> rate[3], 6 -> rate[4], 7 / 14 -> rate[5],
+ * -20 -> cooling[0], 21 -> cooling[1], 22 -> cooling[2]; line rows (-1 / 0 / 1) and FF_COOLING (-21) read none.  Rows of
+ * any other type are refused.  tardis_b200.macro_atom derives the map from the reference's own metadata. */
+typedef struct {
+    int64_t n_transitions;                   /* T: must equal the model's */
+    const int64_t *rate_key;                 /* [T] row of the row's table (not read for line and free-free rows) */
+    const double *energy;                    /* [T] erg: the energy factor of rows 2, 3, -7, 11, 5, 4, 6, 7, 14 (level energy,
+                                                delta_E_yg or ionization energy difference, as the reference picks it) */
+    int64_t n_rate_rows[6];                  /* heights of tb200_continuum_rates.rate[k] */
+    int64_t n_cooling_rows[3];               /* heights of tb200_continuum_rates.cooling[k] */
+} tb200_continuum_rows;
+/* The continuum mode's per-iteration inputs of the macro atom's rows (arguments of ContinuumMacroAtomSolver.solve,
+ * macroatom_solver.py:861-882).  Row (key, shell) of every table at [key * S + shell]. */
+typedef struct {
+    /* [n_rate_rows[k], S]: stim_recomb_corrected_photoionization_rate_coeff, spontaneous_recombination_coeff, coll_deexc_coeff,
+     * coll_exc_coeff, coll_ion_coeff, coll_recomb_coeff.  Unnormalised rows: 2 / 3 / -7: rate * energy
+     * (macroatom_continuum_transitions.py:29,103,178); 11 / 5 / 4 / 6 / 7 / 14: (rate * n_e) * energy (:343,430,514,599,682,763) */
+    const double *rate[6];
+    /* [n_cooling_rows[k], S]: fb_cool_probs_arr.T, coll_exc_cool_arr.T, coll_ion_cool_arr.T; row = cool_rate[s] * cooling[k][key, s] */
+    const double *cooling[3];
+    const double *electron_densities;        /* [S] */
+    const double *ff_cool_rate, *fb_cool_rate, *coll_exc_cool_rate, *coll_ion_cool_rate; /* [S]; FF_COOLING rows = ff_cool_rate */
+    /* [L,S] C-order, both or neither: the beta_Sobolev and stimulated-emission factor the line rows read, as
+     * _solve_next_macroatom_iteration receives them (macroatom_solver.py:1358-1378).  Given, tb200_plasma_state's
+     * level_number_density must be NULL and tau is not rebuilt: the model needs its tau_sobolev from tb200_set_model. */
+    const double *beta_sobolev, *stimulated_emission_factor;
+} tb200_continuum_rates;
 typedef struct {
     int64_t n_lines, n_levels;
     const int64_t *lines_lower_level_index, *lines_upper_level_index; /* [L] rows of the level arrays */
@@ -344,9 +378,12 @@ typedef struct {
     const double *energy_lower, *energy_upper; /* [L] erg: levels.energy of the line's lower / upper level */
     /* constants as the reference's modules compute them (tau_sobolev.py:9-18, macroatom_line_transitions.py:7-11) */
     double sobolev_coefficient, c_einstein, c, h;
+    /* Continuum mode (config.continuum_processes_enabled): required there, refused on any other model.  Checked (types,
+     * keys against the table heights, T) before anything is allocated. */
+    const tb200_continuum_rows *continuum_rows;
 } tb200_atomic_data;
 typedef struct {
-    const double *level_number_density;      /* [n_levels, S] C-order */
+    const double *level_number_density;      /* [n_levels, S] C-order (NULL with tb200_continuum_rates.beta_sobolev) */
     double time_explosion;                   /* s (not read in the nonhomologous mode) */
     const double *j_blues;                   /* [L,S] C-order, or NULL = the table tb200_solve_radiation_field left in HBM
                                                 (only read by the macro atom's internal-up rows) */
@@ -355,11 +392,19 @@ typedef struct {
      * instead of ... * time_explosion * ...  A shell with velocity_gradient < 0 has tau < 0 (and beta > 1), as in the
      * reference; velocity_gradient == 0 is the reference's "Some tau_sobolevs are nan, inf, -inf" error. */
     const double *velocity_gradient;         /* [S], 1/s */
+    /* Continuum mode: required there, refused on any other model.  tau / beta / stim are built as in the homologous mode;
+     * then every row of the macro atom (line rows as above, continuum rows from these tables and the row map of
+     * tb200_set_atomic_data) and their normalisation (macroatom_solver.py:709-739: pandas' Kahan group sum per source
+     * block, NaN addends skipped, then p / sum with NaN -> 0).  The normalised table stays in HBM for
+     * tb200_build_absorbing_markov with transition_probabilities == NULL; until that runs, transport refuses to run. */
+    const tb200_continuum_rates *continuum;
 } tb200_plasma_state;
 int tb200_set_atomic_data(tb200_engine *engine, const tb200_atomic_data *atomic);
 int tb200_build_opacity(tb200_engine *engine, const tb200_plasma_state *plasma);
 /* the tables as the reference would hold them on the host (tests / callers that want them); any pointer may be NULL.
- * transition_probabilities needs the option "keep_opacity_tables" = 1 (the kernels turn the table into running sums in place). */
+ * transition_probabilities needs the option "keep_opacity_tables" = 1 (the kernels turn the table into running sums in place).
+ * In the continuum mode it is the normalised table of the last tb200_build_opacity, refused if that build kept none (the
+ * deactivation table is tb200_download_absorbing_markov's). */
 int tb200_download_opacity(tb200_engine *engine, double *tau_sobolev /* [L,S] */, double *beta_sobolev /* [L,S] */,
                            double *stimulated_emission_factor /* [L,S] */, double *transition_probabilities /* [T,S] */);
 
@@ -378,7 +423,8 @@ typedef struct {
     int64_t n_transitions;                       /* T, as in the model */
     const double *transition_probabilities;      /* normalised (macroatom_solver.py:709-739): (row, shell) at
                                                     [t*tp_transition_stride + s*tp_shell_stride] */
-    int64_t tp_transition_stride, tp_shell_stride;
+    int64_t tp_transition_stride, tp_shell_stride;   /* transition_probabilities == NULL: the table tb200_build_opacity left
+                                                    in HBM (refused if none was built since the last tb200_set_model) */
     const int64_t *source_level_idx, *destination_level_idx, *transition_type; /* [T]; rows with type >= 0 are internal.
                                                     transition_type must equal the model's (the transport reads the rows by it);
                                                     destination_level_idx is read for the internal rows only */

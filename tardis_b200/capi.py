@@ -113,6 +113,18 @@ class RadfieldParams(C.Structure):
 _pu8 = C.POINTER(C.c_uint8)
 
 
+class ContinuumRows(C.Structure):
+    """tb200_continuum_rows"""
+    _fields_ = [("n_transitions", C.c_int64), ("rate_key", _pi), ("energy", _pd), ("n_rate_rows", C.c_int64 * 6),
+                ("n_cooling_rows", C.c_int64 * 3)]
+
+
+class ContinuumRates(C.Structure):
+    """tb200_continuum_rates"""
+    _fields_ = [("rate", _pd * 6), ("cooling", _pd * 3), ("electron_densities", _pd), ("ff_cool_rate", _pd), ("fb_cool_rate", _pd),
+                ("coll_exc_cool_rate", _pd), ("coll_ion_cool_rate", _pd), ("beta_sobolev", _pd), ("stimulated_emission_factor", _pd)]
+
+
 class AtomicData(C.Structure):
     """tb200_atomic_data"""
     _fields_ = [
@@ -120,12 +132,14 @@ class AtomicData(C.Structure):
         ("g", _pd), ("metastability", _pu8), ("nlte_line", _pu8), ("wavelength_f_lu", _pd), ("f_lu", _pd), ("f_ul", _pd),
         ("energy_lower", _pd), ("energy_upper", _pd),
         ("sobolev_coefficient", C.c_double), ("c_einstein", C.c_double), ("c", C.c_double), ("h", C.c_double),
+        ("continuum_rows", C.POINTER(ContinuumRows)),
     ]
 
 
 class PlasmaState(C.Structure):
     """tb200_plasma_state"""
-    _fields_ = [("level_number_density", _pd), ("time_explosion", C.c_double), ("j_blues", _pd), ("velocity_gradient", _pd)]
+    _fields_ = [("level_number_density", _pd), ("time_explosion", C.c_double), ("j_blues", _pd), ("velocity_gradient", _pd),
+                ("continuum", C.POINTER(ContinuumRates))]
 
 
 class MarkovInput(C.Structure):

@@ -11,6 +11,7 @@
 
 #include "../../include/tardis_b200.h"
 #include "continuum_bins.cuh"
+#include "continuum_macro_build.cuh"
 #include "transport_kernel.cuh"
 #include "source_function.cuh"
 #include "packet_source.cuh"
@@ -117,6 +118,14 @@ struct tb200_engine {
     DBuf<double> mk_p_t, mk_q, mk_r, mk_c, mk_keep;  // normalised input [S][tpad]; q [S][n]; pivot row / column; kept X
     DBuf<int> mk_type, mk_dest, mk_err;
     int mk_keep_n = 0;              // n of the kept X (0: none)
+    bool mk_resident = false;       // mk_p_t holds the normalised table of a tb200_build_opacity since the last tb200_set_model
+    // continuum macro atom's rows built on the device (continuum_macro_build.cuh): the row map of tb200_set_atomic_data
+    // (table offset + key * S of every row, -1: none; energy), the per-iteration tables and shell arrays, the kept table
+    int ct_T = -1;                  // T of the row map (-1: none)
+    long long ct_base[tbcm::N_TABLES + 1] = {};  // start of each table in ct_tab, in units of S doubles
+    DBuf<long long> ct_off;
+    DBuf<double> ct_energy, ct_tab, ct_shell, op_cont_tp_t;
+    bool op_cont_valid = false;     // op_cont_tp_t holds the kept normalised table of the last continuum tb200_build_opacity
     // global frequency bins of the bound-free opacity / estimators (continuum_bins.cuh)
     int cont_bins = 0, cb_n_gkeys = 0;
     long long cb_gkey_min = 0;
@@ -225,6 +234,7 @@ void tb200_destroy(tb200_engine *en) {
     en->ff_factor.release(); en->chi_bf_t.release(); en->emiss_t.release(); en->markov_cum.release(); en->pi_refs.release(); en->pi_act.release();
     en->mk_p_t.release(); en->mk_q.release(); en->mk_r.release(); en->mk_c.release(); en->mk_keep.release();
     en->mk_type.release(); en->mk_dest.release(); en->mk_err.release();
+    en->ct_off.release(); en->ct_energy.release(); en->ct_tab.release(); en->ct_shell.release(); en->op_cont_tp_t.release();
     en->line2macro.release(); en->block_edge.release(); en->ttype.release(); en->dest.release(); en->tline.release();
     en->est.release(); en->in_r.release(); en->in_nu.release(); en->in_mu.release(); en->in_energy.release();
     en->out_nu.release(); en->out_energy.release(); en->seeds64.release(); en->seed32.release(); en->x397.release(); en->ps_l_array.release(); en->ps_rejected.release(); en->ps_count.release();
@@ -379,6 +389,9 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     en->opacity_pending = false;
     en->markov_pending = false;
     en->mk_keep_n = 0;
+    en->mk_resident = false;
+    en->op_cont_valid = false;
+    en->ct_T = -1;  // the row map holds offsets for this model's S and was checked against its types: give it again
     if (m->tau_sobolev) {
         if ((r = upload_strided_table(en, m->tau_sobolev, L, S, m->tau_line_stride, m->tau_shell_stride, en->lpad, en->tau_t))) return r;
     } else {  // built on the device by tb200_build_opacity
@@ -1762,7 +1775,93 @@ __global__ void opacity_normalize_kernel(double *tp_t, const int *block_edge, in
         row[t] = isnan(q) ? 0.0 : q;
     }
 }
+// The continuum mode's rows (continuum_macro_build.cuh), one thread per (shell, row) over [S][tpad]: line rows as in
+// opacity_row_kernel, continuum rows from the row map and the per-iteration tables.
+__global__ void continuum_row_kernel(tbo::Constants K, const int *ttype, const int *tline, const long long *ct_off, const double *ct_energy,
+                                     const double *ct_tab, const double *ct_shell, const double *beta_t, const double *stim_t,
+                                     const double *jblues_t, const double *nu, const double *f_ul, const double *f_lu, const double *e_lo,
+                                     const double *e_up, int n_rows, int tpad, int lpad, int n_shells, double *p_t) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n_shells * tpad) return;
+    const int s = (int)(i / tpad), t = (int)(i % tpad);
+    double p = 0.0;
+    if (t < n_rows) {
+        const int type = ttype[t];
+        if (tbcm::is_line_row(type)) {
+            const int l = tline[t];
+            const size_t c = (size_t)s * lpad + l;
+            p = tbo::raw_probability(K, type, beta_t[c], nu[l], f_ul[l], f_lu[l], e_lo[l], e_up[l], stim_t[c], type == 1 ? jblues_t[c] : 0.0);
+        } else {
+            const long long off = ct_off[t];
+            p = tbcm::continuum_probability(type, off >= 0 ? ct_tab[off + s] : 0.0, ct_shell[s], ct_energy[t],
+                                            ct_shell[(size_t)tbcm::cooling_rate(type) * n_shells + s]);
+        }
+    }
+    p_t[i] = p;
+}
+// normalize_transition_probabilities of the continuum mode: one thread per (shell, source block)
+__global__ void continuum_normalize_kernel(double *p_t, const int *block_edge, int n_blocks, int n_shells, int tpad) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n_blocks * n_shells) return;
+    const int shell = (int)(i / n_blocks), block = (int)(i % n_blocks);
+    tbcm::normalize_block(p_t + (size_t)shell * tpad, block_edge[block], block_edge[block + 1]);
+}
 }  // namespace
+
+// The continuum row map of tb200_set_atomic_data, checked against the model's rows before anything is allocated.
+static int set_continuum_rows(tb200_engine *en, const tb200_continuum_rows *cr) {
+    if (!en->continuum) return fail(TB200_ERR_INVALID, "atomic data: continuum_rows is the continuum mode's row map; this model has no continuum");
+    if (cr->n_transitions != en->T)
+        return fail(TB200_ERR_INVALID, "continuum_rows: n_transitions " + std::to_string(cr->n_transitions) + " differs from the model's " + std::to_string(en->T));
+    if (!cr->rate_key || !cr->energy) return fail(TB200_ERR_INVALID, "continuum_rows: rate_key or energy is NULL");
+    const int T = en->T, S = en->S;
+    long long height[tbcm::N_TABLES];
+    for (int k = 0; k < tbcm::N_TABLES; k++) {
+        height[k] = k < 6 ? cr->n_rate_rows[k] : cr->n_cooling_rows[k - 6];
+        if (height[k] < 0) return fail(TB200_ERR_INVALID, "continuum_rows: negative table height");
+    }
+    std::vector<int> tt((size_t)(T > 0 ? T : 1));
+    CK(cudaMemcpy(tt.data(), en->ttype.p, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost));
+    long long base[tbcm::N_TABLES + 1];
+    base[0] = 0;
+    for (int k = 0; k < tbcm::N_TABLES; k++) base[k + 1] = base[k] + height[k];
+    std::vector<long long> off((size_t)(T > 0 ? T : 1), -1);
+    for (int t = 0; t < T; t++) {
+        const int tab = tbcm::row_table(tt[(size_t)t]);
+        if (tab == tbcm::BAD_TYPE)
+            return fail(TB200_ERR_INVALID, "continuum_rows: row " + std::to_string(t) + " has transition_type " + std::to_string(tt[(size_t)t]) +
+                                               ", which the continuum macro atom does not build");
+        if (tab == tbcm::NO_TABLE) continue;
+        const long long key = cr->rate_key[t];
+        if (key < 0 || key >= height[tab])
+            return fail(TB200_ERR_INVALID, "continuum_rows: rate_key " + std::to_string(key) + " of row " + std::to_string(t) + " (type " +
+                                               std::to_string(tt[(size_t)t]) + ") is outside its table of " + std::to_string(height[tab]) + " rows");
+        off[(size_t)t] = (base[tab] + key) * S;
+    }
+    int r;
+    if ((r = en->ct_off.ensure(off.size())) || (r = en->ct_energy.ensure(off.size()))) return r;
+    CK(cudaMemcpy(en->ct_off.p, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(en->ct_energy.p, cr->energy, (size_t)T * sizeof(double), cudaMemcpyHostToDevice));
+    for (int k = 0; k <= tbcm::N_TABLES; k++) en->ct_base[k] = base[k];
+    en->ct_T = T;
+    return TB200_OK;
+}
+
+// The per-iteration continuum tables of tb200_build_opacity into ct_tab / ct_shell (checked by the caller).
+static int upload_continuum_rates(tb200_engine *en, const tb200_continuum_rates *cr) {
+    const int S = en->S;
+    int r;
+    if ((r = en->ct_tab.ensure((size_t)std::max(en->ct_base[tbcm::N_TABLES], 1LL) * S)) || (r = en->ct_shell.ensure((size_t)tbcm::SHELL_ARRAYS * S))) return r;
+    for (int k = 0; k < tbcm::N_TABLES; k++) {
+        const long long rows = en->ct_base[k + 1] - en->ct_base[k];
+        const double *src = k < 6 ? cr->rate[k] : cr->cooling[k - 6];
+        if (rows > 0) CK(cudaMemcpyAsync(en->ct_tab.p + en->ct_base[k] * S, src, (size_t)rows * S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+    }
+    const double *shell[tbcm::SHELL_ARRAYS] = {cr->electron_densities, cr->ff_cool_rate, cr->fb_cool_rate, cr->coll_exc_cool_rate, cr->coll_ion_cool_rate};
+    for (int k = 0; k < tbcm::SHELL_ARRAYS; k++)
+        CK(cudaMemcpyAsync(en->ct_shell.p + (size_t)k * S, shell[k], (size_t)S * sizeof(double), cudaMemcpyHostToDevice, en->stream));
+    return TB200_OK;
+}
 
 int tb200_set_atomic_data(tb200_engine *en, const tb200_atomic_data *a) {
     if (!en || !a) return fail(TB200_ERR_INVALID, "bad argument");
@@ -1771,6 +1870,8 @@ int tb200_set_atomic_data(tb200_engine *en, const tb200_atomic_data *a) {
     if (a->n_levels < 1 || !a->lines_lower_level_index || !a->lines_upper_level_index || !a->g || !a->metastability || !a->wavelength_f_lu ||
         !a->f_lu || !a->f_ul || !a->energy_lower || !a->energy_upper)
         return fail(TB200_ERR_INVALID, "atomic data: missing array");
+    if (en->continuum && !a->continuum_rows)
+        return fail(TB200_ERR_INVALID, "atomic data: the continuum mode needs continuum_rows (the row map of its macro atom)");
     CK(cudaSetDevice(en->device));
     const int L = en->L;
     for (int64_t l = 0; l < L; l++)
@@ -1778,6 +1879,7 @@ int tb200_set_atomic_data(tb200_engine *en, const tb200_atomic_data *a) {
             a->lines_upper_level_index[l] >= a->n_levels)
             return fail(TB200_ERR_INVALID, "atomic data: level index out of range");
     int r;
+    if (a->continuum_rows && (r = set_continuum_rows(en, a->continuum_rows))) return r;  // a refused map keeps the previous one
     en->n_levels = a->n_levels;
     if ((r = upload_i64_as_i32(en, a->lines_lower_level_index, L, en->at_lower)) || (r = upload_i64_as_i32(en, a->lines_upper_level_index, L, en->at_upper))) return r;
     if ((r = en->at_g.ensure(a->n_levels)) || (r = en->at_meta.ensure(a->n_levels)) || (r = en->at_nlte.ensure(L)) || (r = en->at_wfl.ensure(L)) ||
@@ -1798,10 +1900,31 @@ int tb200_set_atomic_data(tb200_engine *en, const tb200_atomic_data *a) {
 }
 
 int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
-    if (!en || !p || !p->level_number_density) return fail(TB200_ERR_INVALID, "bad argument");
+    // continuum rates with beta / stim: the line rows read the caller's tables, tau is the model's (not rebuilt)
+    const bool host_lines = p && p->continuum && (p->continuum->beta_sobolev || p->continuum->stimulated_emission_factor);
+    if (!en || !p || (!p->level_number_density && !host_lines)) return fail(TB200_ERR_INVALID, "bad argument");
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if (!en->have_atomic) return fail(TB200_ERR_NO_MODEL, "tb200_set_atomic_data has not been called");
-    if (en->continuum) return fail(TB200_ERR_INVALID, "the continuum mode's tables are not built on the device");
+    if (!en->continuum && p->continuum) return fail(TB200_ERR_INVALID, "continuum: the continuum mode's rates; this model has no continuum");
+    if (en->continuum) {
+        const tb200_continuum_rates *cr = p->continuum;
+        if (!cr) return fail(TB200_ERR_INVALID, "the continuum mode's macro atom needs continuum (its rates of this iteration)");
+        if (host_lines) {
+            if (!cr->beta_sobolev || !cr->stimulated_emission_factor)
+                return fail(TB200_ERR_INVALID, "continuum: beta_sobolev and stimulated_emission_factor go together");
+            if (p->level_number_density)
+                return fail(TB200_ERR_INVALID, "continuum: with beta_sobolev given, level_number_density must be NULL (tau is not rebuilt)");
+            if (en->opacity_pending)
+                return fail(TB200_ERR_INVALID, "continuum: beta_sobolev given, but the model has no tau_sobolev (tb200_set_model got NULL)");
+        }
+        if (en->ct_T != en->T) return fail(TB200_ERR_NO_MODEL, "the continuum mode needs tb200_set_atomic_data with continuum_rows for this model");
+        if (!cr->electron_densities || !cr->ff_cool_rate || !cr->fb_cool_rate || !cr->coll_exc_cool_rate || !cr->coll_ion_cool_rate)
+            return fail(TB200_ERR_INVALID, "continuum: a per-shell array is NULL");
+        for (int k = 0; k < tbcm::N_TABLES; k++)
+            if (en->ct_base[k + 1] > en->ct_base[k] && !(k < 6 ? cr->rate[k] : cr->cooling[k - 6]))
+                return fail(TB200_ERR_INVALID, std::string("continuum: ") + (k < 6 ? "rate[" : "cooling[") + std::to_string(k < 6 ? k : k - 6) +
+                                                   "] is NULL but the row map reads it");
+    }
     const bool need_jblues = en->have_macro && en->cfg.line_interaction_type == 2;
     if (need_jblues && !p->j_blues && !en->rf_valid)
         return fail(TB200_ERR_INVALID, "j_blues is NULL and tb200_solve_radiation_field has not left a table in HBM");
@@ -1814,10 +1937,14 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
     const int S = en->S, L = en->L, lpad = en->lpad;
     int r;
     cudaStream_t st = en->stream;
-    if ((r = en->op_lnd.ensure((size_t)en->n_levels * S)) || (r = en->op_beta_t.ensure((size_t)S * lpad)) || (r = en->op_stim_t.ensure((size_t)S * lpad))) return r;
-    CK(cudaMemcpyAsync(en->op_lnd.p, p->level_number_density, (size_t)en->n_levels * S * sizeof(double), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(en->error.p, 0, sizeof(int), st));
-    {
+    if (host_lines) {
+        if ((r = upload_strided_table(en, p->continuum->beta_sobolev, L, S, S, 1, lpad, en->op_beta_t)) ||
+            (r = upload_strided_table(en, p->continuum->stimulated_emission_factor, L, S, S, 1, lpad, en->op_stim_t)))
+            return r;
+    } else {
+        if ((r = en->op_lnd.ensure((size_t)en->n_levels * S)) || (r = en->op_beta_t.ensure((size_t)S * lpad)) || (r = en->op_stim_t.ensure((size_t)S * lpad))) return r;
+        CK(cudaMemcpyAsync(en->op_lnd.p, p->level_number_density, (size_t)en->n_levels * S * sizeof(double), cudaMemcpyHostToDevice, st));
         const long long total = (long long)S * lpad;
         const unsigned grid = (unsigned)((total + 255) / 256);
         if (en->nonhomologous) {
@@ -1840,6 +1967,32 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
         }
         if (!need_jblues) jb = en->op_stim_t.p;  // never read (no internal-up rows); any mapped table
         const long long total = (long long)S * en->tpad;
+        if (en->continuum) {  // into the Markov build's input; tp_t keeps the deactivation table until that build
+            en->mk_resident = false;
+            if ((r = en->mk_p_t.ensure((size_t)S * en->tpad + TABLE_SLACK)) || (r = upload_continuum_rates(en, p->continuum))) return r;
+            continuum_row_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(en->op_const, en->ttype.p, en->tline.p, en->ct_off.p,
+                en->ct_energy.p, en->ct_tab.p, en->ct_shell.p, en->op_beta_t.p, en->op_stim_t.p, jb, en->nu_line.p, en->at_ful.p, en->at_flu.p,
+                en->at_elo.p, en->at_eup.p, en->T, en->tpad, lpad, S, en->mk_p_t.p);
+            const long long nb = (long long)en->n_blocks * S;
+            continuum_normalize_kernel<<<(unsigned)((nb + 127) / 128), 128, 0, st>>>(en->mk_p_t.p, en->block_edge.p, en->n_blocks, S, en->tpad);
+            en->launches += 2;
+            CK(cudaGetLastError());
+            if (en->keep_opacity_tables) {
+                if ((r = en->op_cont_tp_t.ensure((size_t)S * en->tpad))) return r;
+                CK(cudaMemcpyAsync(en->op_cont_tp_t.p, en->mk_p_t.p, (size_t)S * en->tpad * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            }
+            CK(cudaStreamSynchronize(st));
+            int err = 0;
+            CK(cudaMemcpy(&err, en->error.p, sizeof(int), cudaMemcpyDeviceToHost));
+            if (err == tb::ERR_OPACITY) return fail(TB200_ERR_INVALID, "Some tau_sobolevs are nan, inf, -inf in tau_sobolevs. Something went wrong!");
+            // the chain is built from this table next (tb200_build_absorbing_markov with transition_probabilities == NULL),
+            // which also finishes the tables the kernels read
+            en->op_cont_valid = en->keep_opacity_tables != 0;
+            en->mk_resident = true;
+            en->markov_pending = true;
+            en->opacity_pending = false;
+            return TB200_OK;
+        }
         opacity_row_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(en->op_const, en->ttype.p, en->tline.p, en->op_beta_t.p, en->op_stim_t.p, jb,
             en->nu_line.p, en->at_ful.p, en->at_flu.p, en->at_elo.p, en->at_eup.p, en->T, en->tpad, lpad, S, en->tp_t.p);
         const long long nb = (long long)en->n_blocks * S;
@@ -1881,10 +2034,14 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
         CK(cudaStreamSynchronize(st));
     }
     if (tp) {
-        if (!en->have_macro || !en->op_tp_norm_t.p) return fail(TB200_ERR_INVALID, "transition_probabilities: set the option keep_opacity_tables before tb200_build_opacity");
+        if (en->continuum && !en->op_cont_valid)
+            return fail(TB200_ERR_INVALID, "transition_probabilities: no kept table of a continuum-mode tb200_build_opacity (set the option "
+                                           "keep_opacity_tables before it; the deactivation table is tb200_download_absorbing_markov's)");
+        const double *kept = en->continuum ? en->op_cont_tp_t.p : en->op_tp_norm_t.p;
+        if (!en->have_macro || !kept) return fail(TB200_ERR_INVALID, "transition_probabilities: set the option keep_opacity_tables before tb200_build_opacity");
         if ((r = en->staging.ensure((size_t)en->T * S))) return r;
         const long long cells = (long long)en->T * S;
-        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(en->op_tp_norm_t.p, en->T, S, en->tpad, en->staging.p);
+        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(kept, en->T, S, en->tpad, en->staging.p);
         en->launches++;
         CK(cudaGetLastError());
         CK(cudaMemcpyAsync(tp, en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -1898,8 +2055,11 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
 static int check_markov_input(tb200_engine *en, const tb200_markov_input *in, std::vector<long long> &edges) {
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if (!en->continuum) return fail(TB200_ERR_INVALID, "tb200_build_absorbing_markov needs a continuum-mode model");
-    if (!in->transition_probabilities || !in->source_level_idx || !in->destination_level_idx || !in->transition_type)
+    if (!in->source_level_idx || !in->destination_level_idx || !in->transition_type)
         return fail(TB200_ERR_INVALID, "absorbing Markov chain: an input array is NULL");
+    if (!in->transition_probabilities && !en->mk_resident)
+        return fail(TB200_ERR_INVALID, "absorbing Markov chain: transition_probabilities is NULL and tb200_build_opacity has built no table "
+                                       "since the last tb200_set_model");
     if (in->n_transitions != en->T) return fail(TB200_ERR_INVALID, "absorbing Markov chain: n_transitions differs from the model's");
     if (in->tp_transition_stride < 0 || in->tp_shell_stride < 0) return fail(TB200_ERR_INVALID, "negative strides are not supported");
     const int64_t T = in->n_transitions, n = in->n_states;
@@ -1960,8 +2120,11 @@ int tb200_build_absorbing_markov(tb200_engine *en, const tb200_markov_input *in)
     cudaStream_t st = en->stream;
     en->markov_pending = true;  // until the build below has finished
     en->mk_keep_n = 0;
-    if ((r = upload_strided_table(en, in->transition_probabilities, en->T, S, in->tp_transition_stride, in->tp_shell_stride, en->tpad, en->mk_p_t)) ||
-        (r = upload_i64_as_i32(en, in->transition_type, en->T, en->mk_type)) ||
+    if (in->transition_probabilities) {  // otherwise mk_p_t holds the table tb200_build_opacity left
+        en->mk_resident = false;
+        if ((r = upload_strided_table(en, in->transition_probabilities, en->T, S, in->tp_transition_stride, in->tp_shell_stride, en->tpad, en->mk_p_t))) return r;
+    }
+    if ((r = upload_i64_as_i32(en, in->transition_type, en->T, en->mk_type)) ||
         (r = upload_i64_as_i32(en, in->destination_level_idx, en->T, en->mk_dest)))
         return r;
     const size_t nm = (size_t)S * n * n, sn = (size_t)S * n;

@@ -378,9 +378,11 @@ class Engine:
 
     # ---- opacity build on the device (SURVEY.md §8f rank 3) ----
     def set_atomic_data(self, *, lines_lower_level_index, lines_upper_level_index, g, metastability, wavelength_cm, f_lu, f_ul,
-                        energy_lower, energy_upper, nlte_line=None):
+                        energy_lower, energy_upper, nlte_line=None, continuum_rows=None):
         """`tb200_set_atomic_data`: the static per-line / per-level data of the opacity build (once per simulation, after
-        the first `set_model`)."""
+        the first `set_model`).  `continuum_rows` (continuum mode only, required there): the macro atom's row map, a dict of
+        rate_key [T], energy [T], n_rate_rows (6 heights) and n_cooling_rows (3 heights) -- see tb200_continuum_rows;
+        `tardis_b200.macro_atom.continuum_row_map` derives it from the reference's metadata."""
         a = capi.AtomicData()
         lo, up = _i64(lines_lower_level_index), _i64(lines_upper_level_index)
         gg = _f64(g)
@@ -400,17 +402,35 @@ class Engine:
         a.sobolev_coefficient = float((np.pi * e_esu**2) / (m_e * c))          # tau_sobolev.py:9-18
         a.c_einstein = float(4.0 * (np.pi * e_esu) ** 2 / (c * m_e))           # macroatom_line_transitions.py:9-11
         a.c, a.h = c, h
+        if continuum_rows is not None:
+            key, en = _i64(continuum_rows["rate_key"]), _f64(continuum_rows["energy"])
+            if len(key) != len(en):
+                raise ValueError("continuum_rows: rate_key and energy need one entry per row")
+            cr = capi.ContinuumRows()
+            cr.n_transitions, cr.rate_key, cr.energy = len(key), _iptr(key), _dptr(en)
+            cr.n_rate_rows[:] = [int(v) for v in continuum_rows["n_rate_rows"]]
+            cr.n_cooling_rows[:] = [int(v) for v in continuum_rows["n_cooling_rows"]]
+            keep += [key, en, cr]
+            a.continuum_rows = C.pointer(cr)
         self._check(self._api("set_atomic_data")(self._h, C.byref(a)))
 
-    def build_opacity(self, level_number_density, time_explosion, j_blues=None, velocity_gradient=None):
+    def build_opacity(self, level_number_density, time_explosion, j_blues=None, velocity_gradient=None, continuum=None):
         """`tb200_build_opacity`: tau_Sobolev, beta_Sobolev and the normalised macro-atom probabilities of this iteration, built
         in HBM from the level populations [n_levels, S] (and J_blue: `None` = the table `solve_radiation_field` left resident).
         `velocity_gradient` [S] (1/s): the nonhomologous mode's tau (modes/nonhomologous/tau_sobolev.py:21-75), required for a
-        nonhomologous model, whose `time_explosion` is then not read."""
+        nonhomologous model, whose `time_explosion` is then not read.  `continuum` (continuum mode only, required there): the
+        macro atom's rates of this iteration, a dict of rate (6 arrays [key, S]), cooling (3 arrays [key, S]: the reference's
+        cooling arrays transposed), electron_densities, ff_cool_rate, fb_cool_rate, coll_exc_cool_rate, coll_ion_cool_rate
+        ([S] each), and optionally beta_sobolev / stimulated_emission_factor [L, S] for the line rows (then
+        `level_number_density` is None and tau stays the model's) -- see tb200_continuum_rates.  The normalised table then
+        stays in HBM for `build_absorbing_markov(None, ...)`."""
         p = capi.PlasmaState()
-        lnd = _f64(level_number_density)
-        keep = [lnd]
-        p.level_number_density, p.time_explosion = _dptr(lnd), float(time_explosion)
+        keep = []
+        if level_number_density is not None:  # None: continuum["beta_sobolev"] / ["stimulated_emission_factor"] are given
+            lnd = _f64(level_number_density)
+            keep.append(lnd)
+            p.level_number_density = _dptr(lnd)
+        p.time_explosion = float(time_explosion)
         if j_blues is not None:
             jb = _f64(j_blues)
             keep.append(jb)
@@ -422,6 +442,29 @@ class Engine:
                 raise ValueError(f"velocity_gradient must have one entry per shell ({S})")
             keep.append(g)
             p.velocity_gradient = _dptr(g)
+        if continuum is not None:
+            S = self._model_shape[1]
+            cr = capi.ContinuumRates()
+            tabs = [_f64(t) for t in (*continuum["rate"], *continuum["cooling"])]
+            if len(tabs) != 9 or any(t.ndim != 2 or t.shape[1] != S for t in tabs):
+                raise ValueError(f"continuum: 6 rate and 3 cooling tables [key, {S}] are needed")
+            shell = [_f64(continuum[k]) for k in ("electron_densities", "ff_cool_rate", "fb_cool_rate", "coll_exc_cool_rate", "coll_ion_cool_rate")]
+            if any(a.shape != (S,) for a in shell):
+                raise ValueError(f"continuum: the per-shell arrays need {S} entries")
+            for k in range(6):
+                cr.rate[k] = _dptr(tabs[k])
+            for k in range(3):
+                cr.cooling[k] = _dptr(tabs[6 + k])
+            cr.electron_densities, cr.ff_cool_rate, cr.fb_cool_rate, cr.coll_exc_cool_rate, cr.coll_ion_cool_rate = map(_dptr, shell)
+            keep += [*tabs, *shell, cr]
+            for k in ("beta_sobolev", "stimulated_emission_factor"):
+                if continuum.get(k) is not None:
+                    t = _f64(continuum[k])
+                    if t.shape != (self._model_shape[0], S):
+                        raise ValueError(f"continuum: {k} must be [n_lines, n_shells]")
+                    keep.append(t)
+                    setattr(cr, k, _dptr(t))
+            p.continuum = C.pointer(cr)
         self._check(self._api("build_opacity")(self._h, C.byref(p)))
 
     def download_opacity(self, transition_probabilities=False):
@@ -442,22 +485,27 @@ class Engine:
         """`tb200_build_absorbing_markov`: the absorbing-Markov-chain table X [S, n, n] and the normalised deactivation table
         of this iteration, built in HBM from the normalised transition probabilities [T, S] (may be a strided view) and the
         rows' source / destination state and type (create_absorbing_probs + the second normalisation of the reference's
-        ContinuumMacroAtomSolver).  n_states defaults to max(source_level_idx) + 1."""
-        tp = np.asarray(transition_probabilities, dtype=np.float64)
-        if tp.ndim != 2:
-            raise ValueError("transition_probabilities must be [n_transitions, n_shells]")
-        if any(s < 0 or s % 8 for s in tp.strides):
-            tp = np.ascontiguousarray(tp)
+        ContinuumMacroAtomSolver).  n_states defaults to max(source_level_idx) + 1.  transition_probabilities = None: the
+        table the last continuum-mode `build_opacity` left in HBM."""
         src, dst, tt = _i64(source_level_idx), _i64(destination_level_idx), _i64(transition_type)
-        if not (len(src) == len(dst) == len(tt) == tp.shape[0]):
-            raise ValueError("source_level_idx, destination_level_idx and transition_type need one entry per row")
-        if tp.shape[1] != self._model_shape[1]:
-            raise ValueError("transition_probabilities must have one column per shell of the model")
-        keep = [tp, src, dst, tt]
         m = capi.MarkovInput()
-        m.n_transitions = tp.shape[0]
-        m.transition_probabilities = _dptr(tp)
-        m.tp_transition_stride, m.tp_shell_stride = tp.strides[0] // 8, tp.strides[1] // 8
+        keep = [src, dst, tt]
+        if transition_probabilities is not None:
+            tp = np.asarray(transition_probabilities, dtype=np.float64)
+            if tp.ndim != 2:
+                raise ValueError("transition_probabilities must be [n_transitions, n_shells]")
+            if any(s < 0 or s % 8 for s in tp.strides):
+                tp = np.ascontiguousarray(tp)
+            if tp.shape[0] != len(src):
+                raise ValueError("source_level_idx, destination_level_idx and transition_type need one entry per row")
+            if tp.shape[1] != self._model_shape[1]:
+                raise ValueError("transition_probabilities must have one column per shell of the model")
+            keep.append(tp)
+            m.transition_probabilities = _dptr(tp)
+            m.tp_transition_stride, m.tp_shell_stride = tp.strides[0] // 8, tp.strides[1] // 8
+        if not (len(src) == len(dst) == len(tt)):
+            raise ValueError("source_level_idx, destination_level_idx and transition_type need one entry per row")
+        m.n_transitions = len(src)
         m.source_level_idx, m.destination_level_idx, m.transition_type = _iptr(src), _iptr(dst), _iptr(tt)
         m.n_states = int(src.max()) + 1 if n_states is None else int(n_states)
         self._check(self._api("build_absorbing_markov")(self._h, C.byref(m)))

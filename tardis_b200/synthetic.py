@@ -574,3 +574,144 @@ def make_nonhomologous_velocities(model: Model, amplitude: float = 0.08, seed: i
             k = (len(v) - 1) // 2
             v[k] = v[k + 1] * (1.0 + 0.5 * amplitude)
     return dataclasses.replace(model, v_inner=np.ascontiguousarray(v[:-1]), v_outer=np.ascontiguousarray(v[1:]))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Inputs of the continuum (IIP) macro atom's per-iteration rows (ContinuumMacroAtomSolver.solve,
+# opacities/macro_atom/macroatom_solver.py:861-1020), in the reference's index layout
+# ---------------------------------------------------------------------------------------------------------------------
+@dataclass
+class ContinuumRateInputs:
+    """Static atomic data as the reference's ContinuumMacroAtomSolver takes it (levels, lines, photoionization_data,
+    ionization_energies: pandas objects indexed by (atomic_number, ion_number, level_number[_lower, _upper])), the same
+    data as arrays for the engine's opacity build (`atomic`, rows of `levels`), and per iteration the level populations,
+    J_blue and the continuum rates / cooling arrays of `solve` (`rates[i]`: keyword arguments of `solve` without
+    mean_intensities_blue_wing / beta_sobolevs / stimulated_emission_factors, which follow from the populations)."""
+
+    levels: object                 # DataFrame [n_levels] energy, g, metastable
+    lines: object                  # DataFrame [L] nu, f_lu, f_ul, wavelength_cm, line_id (descending nu)
+    photoionization_data: object   # DataFrame, two cross-section points per level with a bound-free continuum
+    ionization_energies: object    # Series indexed by the next ion's ground state
+    atomic: AtomicData             # the line / level arrays (macro-row fields empty: the reference's metadata fills them)
+    plasma: list                   # [PlasmaState] per iteration
+    rates: list                    # [dict] per iteration
+
+
+def make_continuum_rate_inputs(n_shells: int, n_h_levels: int = 8, n_he_levels: int = 6, seed: int = MODEL_SEED + 10,
+                               n_lines: int | None = None, n_iterations: int = 2, shuffle_rates: bool = False,
+                               zero_levels: int = 0, infinite_rate: bool = False) -> ContinuumRateInputs:
+    """Hydrogen (H I levels + the H II ground state) and helium (He I levels + the He II ground state).  Every H I level and
+    the lower half of He I have a bound-free continuum; collisional (de-)excitation joins every pair of levels of an ion,
+    collisional ionization / recombination every level with a continuum; collisional-excitation cooling points at the
+    pair's upper level (so destinations repeat).  Rates are log-uniform per (key, shell) and differ per iteration.
+    `shuffle_rates`: the photoionization / recombination / collisional-ionization frames are stored in a permuted row order
+    (their labels still name the level), so a lookup by position instead of by label reads another level's rate.
+    `zero_levels`: that many H I levels get all-zero rates, populations and lines removed -- empty source blocks.
+    `infinite_rate`: one photoionization rate is +inf in shell 0 of the second iteration (its level's block normalises to
+    0 / inf and inf / inf -> NaN -> 0; a ground-state rate times energy 0 is NaN, which pandas' group sum skips)."""
+    import pandas as pd
+
+    rng = np.random.default_rng(seed)
+    S = n_shells
+    species = [(1, 0, n_h_levels), (1, 1, 1), (2, 0, n_he_levels), (2, 1, 1)]
+    tuples, energy = [], []
+    for a, ion, n in species:
+        e = np.sort(rng.uniform(1e-12, 3e-11, n))
+        e[0] = 0.0
+        for lev in range(n):
+            tuples.append((a, ion, lev))
+            energy.append(e[lev])
+    level_index = pd.MultiIndex.from_tuples(tuples, names=["atomic_number", "ion_number", "level_number"])
+    n_levels = len(tuples)
+    g = (rng.integers(1, 9, n_levels) * 2 - 1).astype(np.float64)
+    metastable = rng.random(n_levels) < 0.1
+    levels = pd.DataFrame({"energy": np.array(energy), "g": g, "metastable": metastable}, index=level_index)
+    row_of = {t: i for i, t in enumerate(tuples)}
+    zero = set()
+    if zero_levels:
+        zero = {(1, 0, int(lev)) for lev in rng.choice(np.arange(1, n_h_levels), zero_levels, replace=False)}
+
+    # lines: every pair of an ion's levels (a random subset when n_lines is given), sorted by descending frequency
+    pairs = [(a, ion, lo, up) for a, ion, n in species for lo in range(n) for up in range(lo + 1, n)
+             if (a, ion, lo) not in zero and (a, ion, up) not in zero]
+    if n_lines is not None and n_lines < len(pairs):
+        pairs = [pairs[i] for i in np.sort(rng.choice(len(pairs), n_lines, replace=False))]
+    e_lo = np.array([levels.energy.iloc[row_of[(a, i, lo)]] for a, i, lo, up in pairs])
+    e_up = np.array([levels.energy.iloc[row_of[(a, i, up)]] for a, i, lo, up in pairs])
+    nu = (e_up - e_lo) / H_PLANCK
+    order = np.argsort(-nu, kind="stable")
+    pairs = [pairs[i] for i in order]
+    nu = nu[order]
+    L = len(pairs)
+    lo_row = np.array([row_of[(a, i, lo)] for a, i, lo, up in pairs], dtype=np.int64)
+    up_row = np.array([row_of[(a, i, up)] for a, i, lo, up in pairs], dtype=np.int64)
+    f_lu = 10 ** rng.uniform(-3, 0, L)
+    f_ul = f_lu * g[lo_row] / g[up_row]
+    line_index = pd.MultiIndex.from_tuples(pairs, names=["atomic_number", "ion_number", "level_number_lower", "level_number_upper"])
+    lines = pd.DataFrame({"nu": nu, "f_lu": f_lu, "f_ul": f_ul, "wavelength_cm": C_SPEED_OF_LIGHT / nu,
+                          "line_id": np.arange(L, dtype=np.int64)}, index=line_index)
+    atomic = AtomicData(lo_row, up_row, g, levels.energy.to_numpy().copy(), metastable, nu.copy(), C_SPEED_OF_LIGHT / nu, f_lu, f_ul,
+                        np.zeros(L, dtype=bool), *(np.zeros(0, dtype=np.int64) for _ in range(6)))
+
+    # continua and collisions
+    bf = [(1, 0, lev) for lev in range(n_h_levels)] + [(2, 0, lev) for lev in range((n_he_levels + 1) // 2)]
+    bf_index = pd.MultiIndex.from_tuples(bf, names=["atomic_number", "ion_number", "level_number"])
+    pi_rows = pd.MultiIndex.from_tuples([t for t in bf for _ in range(2)], names=bf_index.names)
+    photoionization_data = pd.DataFrame({"nu": rng.uniform(1e15, 4e15, len(pi_rows)), "x_sect": rng.uniform(1e-19, 6e-18, len(pi_rows))},
+                                        index=pi_rows)
+    ion_e = {(1, 1, 0): 2.18e-11, (2, 1, 0): 3.94e-11}
+    ionization_energies = pd.Series(ion_e).rename_axis(["atomic_number", "ion_number", "level_number"])
+    coll = [(a, ion, lo, up) for a, ion, n in species if ion == 0 for lo in range(n) for up in range(lo + 1, n)]
+    coll_index = pd.MultiIndex.from_tuples(coll, names=["atomic_number", "ion_number", "level_number_lower", "level_number_upper"])
+    delta_E_yg = pd.Series([levels.energy.iloc[row_of[(a, i, up)]] - levels.energy.iloc[row_of[(a, i, lo)]] for a, i, lo, up in coll],
+                           index=coll_index)
+    exc_dest = pd.MultiIndex.from_tuples([(a, i, up) for a, i, lo, up in coll], names=bf_index.names)
+    perm = rng.permutation(len(bf)) if shuffle_rates else np.arange(len(bf))
+    columns = pd.RangeIndex(S)
+
+    def frame(keys, index, lo=-14.0, hi=-8.0):
+        v = 10 ** rng.uniform(lo, hi, (len(index), S))
+        for k, key in enumerate(keys):
+            if zero.intersection(key):
+                v[k] = 0.0
+        return pd.DataFrame(v, index=index, columns=columns)
+
+    def by_level(lo=-14.0, hi=-8.0):
+        f = frame([(t,) for t in bf], bf_index, lo, hi)
+        return f.iloc[perm]
+
+    plasma, rates = [], []
+    for it in range(n_iterations):
+        t = rng.uniform(6e3, 1.4e4, S)
+        lnd = g[:, None] * np.exp(-levels.energy.to_numpy()[:, None] / (K_BOLTZMANN * t[None, :])) * np.geomspace(1e9, 1e7, S)[None, :]
+        lnd *= np.exp(rng.normal(0.0, 0.3, S))[None, :]   # per shell: no inverted pairs, so every probability is >= 0
+        for key in zero:
+            lnd[row_of[key]] = 0.0
+        plasma.append(PlasmaState(np.ascontiguousarray(lnd), np.ascontiguousarray(10 ** rng.uniform(-9, -5, (L, S))), 1.0e6 * (1 + it)))
+        coll_keys = [((a, i, lo), (a, i, up)) for a, i, lo, up in coll]
+        pi = by_level()
+        if infinite_rate and it == n_iterations - 1:
+            pi.iloc[int(np.flatnonzero(perm == 0)[0]), 0] = np.inf      # the H ground state (energy 0): inf * 0 = NaN
+            pi.iloc[int(np.flatnonzero(perm == 1)[0]), 0] = np.inf      # the first excited H level: its block -> 0 / inf
+        r = dict(
+            stim_recomb_corrected_photoionization_rate_coeff=pi,
+            spontaneous_recombination_coeff=by_level(-13.0, -11.0),
+            coll_deexc_coeff=frame(coll_keys, coll_index, -9.0, -6.0),
+            coll_exc_coeff=frame(coll_keys, coll_index, -12.0, -7.0),
+            coll_ion_coeff=by_level(-16.0, -10.0),
+            coll_recomb_coeff=by_level(-22.0, -18.0),
+            electron_densities=pd.Series(np.geomspace(1e9, 1e8, S) * rng.uniform(0.8, 1.2, S), index=columns),
+            delta_E_yg=delta_E_yg,
+            coll_exc_cool_rate=10 ** rng.uniform(-12, -9, S),
+            coll_exc_cool_arr=rng.dirichlet(np.ones(len(coll)), S),
+            coll_exc_cool_destinations=exc_dest,
+            coll_ion_cool_rate=10 ** rng.uniform(-12, -9, S),
+            coll_ion_cool_arr=rng.dirichlet(np.ones(len(bf)), S),
+            fb_cool_rate=10 ** rng.uniform(-12, -9, S),
+            fb_cool_probs_arr=rng.dirichlet(np.ones(len(bf)), S),
+            ff_cool_rate=10 ** rng.uniform(-12, -9, S),
+        )
+        for k in ("coll_exc_cool_arr", "coll_ion_cool_arr", "fb_cool_probs_arr"):
+            r[k][:, 0] = 0.0 if it == 0 else r[k][:, 0]   # a zero cooling channel in the first iteration
+        rates.append(r)
+    return ContinuumRateInputs(levels, lines, photoionization_data, ionization_energies, atomic, plasma, rates)
