@@ -186,7 +186,7 @@ int tb200_run(tb200_engine *engine, const tb200_packets *packets, tb200_outputs 
 int tb200_run_resident(tb200_engine *engine, tb200_outputs *outputs);
 
 /* ---- the same work as separate stages, for callers that keep data resident in HBM ---- */
-int tb200_upload_packets(tb200_engine *engine, const tb200_packets *packets); /* H2D + per-packet RNG seed expansion */
+int tb200_upload_packets(tb200_engine *engine, const tb200_packets *packets); /* H2D (each transport expands the seeds) */
 
 /* ---- device-side packet source (SURVEY.md §8f rank 1): the packets never exist on the host ----
  * Fills the engine's resident packet arrays with what BlackBodySimpleSource.create_packets(no_of_packets, seed_offset)

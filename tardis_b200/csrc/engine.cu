@@ -144,7 +144,7 @@ struct tb200_engine {
     DBuf<unsigned long long> ps_rejected;
     DBuf<unsigned> ps_count;
     DBuf<unsigned> seed32, x397, order_hist;
-    DBuf<int> order;
+    DBuf<tb::StartRecord> start_rec;         // by processing slot (tb::StartRecord), written by the ordering pass
     // radiation-field solve (radfield.cuh): resident results + scratch for host-supplied estimators
     DBuf<double> rf_shell;   // [5 S]: t_rad, w, norm, j, nu_bar (the last two only with host-supplied estimators)
     DBuf<double> rf_volume, rf_jblues_t, rf_in_t;  // [S]; [S][lpad] normalised J_blue (shell-major); [S][lpad] uploaded estimator
@@ -238,7 +238,7 @@ void tb200_destroy(tb200_engine *en) {
     en->line2macro.release(); en->block_edge.release(); en->ttype.release(); en->dest.release(); en->tline.release();
     en->est.release(); en->in_r.release(); en->in_nu.release(); en->in_mu.release(); en->in_energy.release();
     en->out_nu.release(); en->out_energy.release(); en->seeds64.release(); en->seed32.release(); en->x397.release(); en->ps_l_array.release(); en->ps_rejected.release(); en->ps_count.release();
-    en->order.release(); en->order_hist.release();
+    en->start_rec.release(); en->order_hist.release();
     en->at_lower.release(); en->at_upper.release(); en->at_meta.release(); en->at_nlte.release(); en->at_g.release(); en->at_wfl.release();
     en->at_flu.release(); en->at_ful.release(); en->at_elo.release(); en->at_eup.release(); en->op_lnd.release(); en->op_beta_t.release();
     en->op_stim_t.release(); en->op_tp_norm_t.release(); en->op_dvdr.release();
@@ -615,8 +615,8 @@ int tb200_upload_packets(tb200_engine *en, const tb200_packets *pk) {
     CK(cudaMemcpyAsync(en->in_mu.p, pk->initial_mus, n * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->in_energy.p, pk->initial_energies, n * sizeof(double), cudaMemcpyHostToDevice, en->stream));
     CK(cudaMemcpyAsync(en->seeds64.p, pk->packet_seeds, n * sizeof(long long), cudaMemcpyHostToDevice, en->stream));
-    // (the per-packet RNG seed expansion and the processing order are part of every tb200_transport: an MC iteration
-    //  has new packets every time, so a timed step pays for them)
+    // (the processing order, with each packet's start record and RNG seed expansion, is part of every tb200_transport: an
+    //  MC iteration has new packets every time, so a timed step pays for it)
     return TB200_OK;
 }
 
@@ -880,25 +880,11 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
     }
 
     if (n > 0) {
-        // processing order by initial frequency, inside this range (indices are relative to the range)
-        const bool use_order = en->sort_packets != 0;
-        if (use_order) {  // recomputed on every launch: every iteration brings new packets
-            const int shift = 52 - en->sort_bits;
-            const long long okey_min = (en->key_min << tb::NU_KEY_SHIFT) >> shift;
-            const long long okey_max = (((en->key_min + en->n_keys - 1) << tb::NU_KEY_SHIFT) >> shift);
-            const int n_okeys = (int)(okey_max - okey_min + 1);
-            if ((r = en->order.ensure((size_t)en->N)) || (r = en->order_hist.ensure((size_t)n_okeys))) return r;
-            CK(cudaMemsetAsync(en->order_hist.p, 0, (size_t)n_okeys * sizeof(unsigned), en->stream));
-            tb::order_hist_kernel<<<(unsigned)((n + 256 * tb::ORDER_ITEMS - 1) / (256 * tb::ORDER_ITEMS)), 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p);
-            tb::order_scan_kernel<<<1, 1024, 0, en->stream>>>(en->order_hist.p, n_okeys);
-            tb::order_scatter_kernel<<<(unsigned)((n + 256 * tb::ORDER_ITEMS - 1) / (256 * tb::ORDER_ITEMS)), 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p, en->order.p + off);
-            en->launches += 3;
-            CK(cudaGetLastError());
-        }
+        if ((r = en->start_rec.ensure((size_t)en->N))) return r;
         P.n_packets = n;
         P.in_r = en->in_r.p + off; P.in_nu = en->in_nu.p + off; P.in_mu = en->in_mu.p + off; P.in_energy = en->in_energy.p + off;
         P.seed = en->seed32.p + off; P.seed_x397 = en->x397.p + off;
-        P.order = use_order ? en->order.p + off : nullptr;
+        P.start = en->start_rec.p + off;
         P.out_nu = en->out_nu.p + off; P.out_energy = en->out_energy.p + off;
         if (en->track_last) {
             long long *li = en->last_i.p + off; double *ld = en->last_d.p + off; const int64_t N = en->N;
@@ -942,6 +928,39 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
         KERNEL<<<resident_grid, threads, smem, en->stream>>>();                                                            \
     } while (0)
         CK(cudaMemcpyToSymbolAsync(tb::cP, &P, sizeof(P), 0, cudaMemcpyHostToDevice, en->stream));
+        // The processing order by initial frequency, inside this range (indices are relative to the range), recomputed on every
+        // launch (every iteration brings new packets).  It writes each packet's start record at its slot, computed from the
+        // range's packets and the model in cP, and the seed words by packet id (tb::order_scatter_kernel).
+        {
+            const long long *seeds64 = en->seeds64.p + off;
+            unsigned *seed32 = en->seed32.p + off, *x397 = en->x397.p + off;
+            tb::StartRecord *rec = en->start_rec.p + off;
+            if (en->sort_packets) {
+                const int shift = 52 - en->sort_bits;
+                const long long okey_min = (en->key_min << tb::NU_KEY_SHIFT) >> shift;
+                const long long okey_max = (((en->key_min + en->n_keys - 1) << tb::NU_KEY_SHIFT) >> shift);
+                const int n_okeys = (int)(okey_max - okey_min + 1);
+                if ((r = en->order_hist.ensure((size_t)n_okeys))) return r;
+                const unsigned nblk = (unsigned)((n + 256 * tb::ORDER_ITEMS - 1) / (256 * tb::ORDER_ITEMS));
+                CK(cudaMemsetAsync(en->order_hist.p, 0, (size_t)n_okeys * sizeof(unsigned), en->stream));
+                tb::order_hist_kernel<<<nblk, 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p);
+                tb::order_scan_kernel<<<1, 1024, 0, en->stream>>>(en->order_hist.p, n_okeys);
+#define TB_SCATTER(START) \
+    tb::order_scatter_kernel<START><<<nblk, 256, 0, en->stream>>>(en->in_nu.p + off, n, shift, okey_min, n_okeys, en->order_hist.p, seeds64, seed32, x397, rec)
+                if (en->nonhomologous) TB_SCATTER(nh::NhStart);
+                else if (P.full_rel) TB_SCATTER(tb::ClassicStart<true>);
+                else TB_SCATTER(tb::ClassicStart<false>);
+#undef TB_SCATTER
+                en->launches += 3;
+            } else {
+                const unsigned nblk = (unsigned)((n + 255) / 256);
+                if (en->nonhomologous) tb::start_record_kernel<nh::NhStart><<<nblk, 256, 0, en->stream>>>(n, seeds64, seed32, x397, rec);
+                else if (P.full_rel) tb::start_record_kernel<tb::ClassicStart<true>><<<nblk, 256, 0, en->stream>>>(n, seeds64, seed32, x397, rec);
+                else tb::start_record_kernel<tb::ClassicStart<false>><<<nblk, 256, 0, en->stream>>>(n, seeds64, seed32, x397, rec);
+                en->launches++;
+            }
+            CK(cudaGetLastError());
+        }
         if (ev_a) CK(cudaEventRecord(ev_a, en->stream));
         // one kernel per mode, compiled for the CTAs per SM its default runs at (see ctas_per_sm above)
         if (en->nonhomologous) {  // whatever the algorithm / pooled options say
@@ -994,12 +1013,6 @@ static int launch_range(tb200_engine *en, int64_t off, int64_t n, bool first, bo
 }
 
 static int launch_transport(tb200_engine *en, int zero_estimators) {
-    if (en->N > 0) {  // MT19937 seed words of every packet (Rng::start), from the resident 64-bit seeds
-        CK(cudaSetDevice(en->device));
-        tb::seed_expand_kernel<<<(unsigned)((en->N + 255) / 256), 256, 0, en->stream>>>(en->seeds64.p, en->seed32.p, en->x397.p, en->N);
-        en->launches++;
-        CK(cudaGetLastError());
-    }
     int r = launch_range(en, 0, en->N, true, true, zero_estimators, en->ev_start, en->ev_stop);
     if (r) return r;
     CK(cudaEventRecord(en->ev_fin, en->stream));
@@ -1205,8 +1218,6 @@ static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_output
             chk(cudaStreamWaitEvent(en->stream, ev_up[c], 0));
         }
         if (rc) break;
-        tb::seed_expand_kernel<<<(unsigned)((m + 255) / 256), 256, 0, en->stream>>>(en->seeds64.p + lo, en->seed32.p + lo, en->x397.p + lo, m);
-        en->launches++;
         if ((rc = launch_range(en, lo, m, c == 0, c == chunks - 1, 1, ev_k0[c], ev_k1[c]))) break;
         // outputs of this range go back while the next range computes
         chk(cudaStreamWaitEvent(en->d2h_stream, ev_k1[c], 0));

@@ -368,24 +368,34 @@ __device__ __noinline__ void vpacket_volley(const Lane &p, Rng &rng, unsigned lo
     }
 }
 
-// packet_propagation.py:101-126: set_packet_props_partial_relativity at get_velocity, the first line ids, the tracker,
-// the first volley and the synthetic boundary event -1 -> 0
-__device__ __noinline__ void start_packet(NhPacket &q, Rng &rng, long long pid, Counters &c) {
+// packet_propagation.py:101-108: set_packet_props_partial_relativity at get_velocity and the first line id of packet pid,
+// written into its StartRecord by the ordering pass (tb::order_scatter_kernel / tb::start_record_kernel)
+struct NhStart {
+    __device__ __forceinline__ static tb::StartRecord at(long long pid, long long seed64) {
+        const KParams &P = cP;
+        tb::StartRecord s;
+        s.pid = (int)pid;
+        s.r = P.in_r[pid]; s.mu = P.in_mu[pid]; s.nu = P.in_nu[pid]; s.energy = P.in_energy[pid];
+        const uint2 sx = tb::seed_expand(seed64);
+        s.seed = sx.x; s.x397 = sx.y;
+        const double v = vel_at(s.r, 0);
+        const double inv_doppler = tb::inverse_doppler_factor<false>(v, s.mu);
+        s.nu *= inv_doppler; s.energy *= inv_doppler;
+        // L - searchsorted(nu[::-1], comov_nu, 'left') == #lines with nu_line >= comov_nu
+        int next = tb::first_line_below(s.nu * tb::doppler_factor<false>(v, s.mu));
+        if (next == P.n_lines) next -= 1;
+        s.next_line = next;
+        return s;
+    }
+};
+
+// packet_propagation.py:101-126 for the packet at processing slot `slot`: its StartRecord, the second line id, the
+// tracker, the first volley and the synthetic boundary event -1 -> 0
+__device__ __noinline__ void start_packet(NhPacket &q, Rng &rng, long long slot, Counters &c) {
     const KParams &P = cP;
-    const int L = P.n_lines;
     Lane &p = q.p;
-    p.pid = (int)pid;
-    p.r = P.in_r[pid]; p.mu = P.in_mu[pid]; p.nu = P.in_nu[pid]; p.energy = P.in_energy[pid];
-    p.shell = 0; p.status = tb::ST_IN_PROCESS; p.icount = 0; p.bbuf = -1; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
-    rng.start(P.seed[pid], P.seed_x397[pid], (unsigned)pid);
-    const double v = vel_at(p.r, 0);
-    const double inv_doppler = tb::inverse_doppler_factor<false>(v, p.mu);
-    p.nu *= inv_doppler; p.energy *= inv_doppler;
-    // L - searchsorted(nu[::-1], comov_nu, 'left') == #lines with nu_line >= comov_nu
-    int next = tb::first_line_below(p.nu * tb::doppler_factor<false>(v, p.mu));
-    if (next == L) next -= 1;
-    p.next_line = next;
-    q.prev_line = next - 1;
+    const int pid = tb::start_from_record(p, rng, slot);
+    q.prev_line = p.next_line - 1;
     if (P.last_type) {  // TrackerLastInteraction.__init__, tracker_last_interaction.py:55-82
         const double qnan = __longlong_as_double(0x7ff8000000000000ll);
         P.last_type[pid] = -1; P.last_event_id[pid] = 0; P.last_shell[pid] = -1;
@@ -523,13 +533,12 @@ __global__ void __launch_bounds__(256, 2) transport_nonhomologous_kernel() {
     while (*((volatile int *)P.error) == 0) {
         const unsigned long long slot = atomicAdd(P.next_packet, 1ull);
         if (slot >= (unsigned long long)P.n_packets) break;
-        const long long pid = P.order ? (long long)P.order[slot] : (long long)slot;
         // The out-of-line calls get copies (the calling convention of transport_kernel.cuh): an object whose address
         // reaches a real call lives in local memory for its whole life.
         NhPacket q;
         {
             NhPacket lq; Rng lr = rng; Counters lc;
-            start_packet(lq, lr, pid, lc);
+            start_packet(lq, lr, (long long)slot, lc);
             q = lq; rng = lr; tb::flush_rare(lc);
         }
         while (q.p.status == tb::ST_IN_PROCESS) {

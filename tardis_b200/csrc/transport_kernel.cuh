@@ -57,6 +57,18 @@ struct Event {  // == tb200_event
     double radius, before_nu, before_mu, before_energy, after_nu, after_mu, after_energy;
 };
 
+// Everything a packet's start needs, written at the packet's processing slot by the ordering pass (start_record_kernel /
+// order_scatter_kernel): the lab-to-comoving transform of r, mu, nu, energy, the first line id, the 32-bit seed and x[397] of
+// its generator, and the packet id.  A refill then takes consecutive slots with one coalesced 48-byte load per lane where
+// it took a dependent chain (order -> six scattered gathers -> frame transform -> line search).
+struct __align__(16) StartRecord {
+    double r, mu, nu, energy;
+    int next_line;
+    unsigned seed, x397;
+    int pid;
+};
+static_assert(sizeof(StartRecord) == 48, "StartRecord is three 16-byte loads");
+
 struct KParams {
     // ---- geometry + opacity tables (device) ----
     int n_shells, n_lines, lpad;
@@ -96,8 +108,8 @@ struct KParams {
     // ---- packets ----
     long long n_packets;
     const double *in_r, *in_nu, *in_mu, *in_energy;
-    const unsigned *seed, *seed_x397;
-    const int *order;                        // optional processing order (packet ids), or nullptr
+    const unsigned *seed, *seed_x397;        // by packet id: what rng_replay_tier1 replays a packet's first outputs from
+    const StartRecord *start;                // by processing slot (StartRecord)
     int refill_min;                          // refill a warp when this many lanes are free
     int park_min;                           // jump kernel: run the slow phase when this many lanes are parked
     double *out_nu, *out_energy;
@@ -149,7 +161,7 @@ __constant__ KParams cP;
 //   outputs   0..226 : x[n], x[n+1], x[n+397] all come from the Knuth init recurrence -> two running cursors
 //   outputs 227..623 : x[n+397] is an already generated word, read back from the per-lane ring
 //   outputs 624..    : the textbook in-place recurrence on the ring
-// x[397] of each packet's seed is precomputed by seed_expand_kernel.
+// x[397] of each packet's seed is precomputed by the ordering pass (start_fields).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned mt_init_next(unsigned x, unsigned k) { return 1812433253u * (x ^ (x >> 30)) + k; }
 
@@ -261,15 +273,13 @@ struct Rng {
     }
 };
 
-__global__ void seed_expand_kernel(const long long *seeds64, unsigned *seed32, unsigned *x397, long long n) {
-    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    unsigned s = (unsigned)(seeds64[i] & 0xffffffffll);  // np.random.seed takes uint32 (randomimpl.py:213-225)
-    seed32[i] = s;
+// the generator's 32-bit seed and x[397] (Rng::start) from a packet's 64-bit seed
+__device__ __forceinline__ uint2 seed_expand(long long seed64) {
+    const unsigned s = (unsigned)(seed64 & 0xffffffffll);  // np.random.seed takes uint32 (randomimpl.py:213-225)
     unsigned x = s;
 #pragma unroll 4
     for (unsigned k = 1; k <= 397u; k++) x = mt_init_next(x, k);
-    x397[i] = x;
+    return make_uint2(s, x);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1303,35 +1313,53 @@ __device__ __noinline__ void warp_volley(bool active, const Lane &p, Rng &rng, u
 // Pieces of packet_propagation shared by both kernels
 // ------------------------------------------------------------------------------------------
 
-// make_r_packet (modes/montecarlo_transport.py:41-66) + the prologue of packet_propagation
-// (modes/classic/packet_propagation.py:99-122)
+// The packet's record at its processing slot (StartRecord): three 16-byte loads
+__device__ __forceinline__ int start_from_record(Lane &p, Rng &rng, long long slot) {
+    const double2 *rec = reinterpret_cast<const double2 *>(cP.start + slot);
+    const double2 rmu = rec[0], nue = rec[1];
+    const int4 w = reinterpret_cast<const int4 *>(rec)[2];
+    p.pid = w.w; p.r = rmu.x; p.mu = rmu.y; p.nu = nue.x; p.energy = nue.y; p.next_line = w.x;
+    p.shell = 0; p.status = ST_IN_PROCESS; p.icount = 0; p.bbuf = -1; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
+    rng.start((unsigned)w.y, (unsigned)w.z, (unsigned)w.w);
+    return w.w;
+}
+
+// make_r_packet (modes/montecarlo_transport.py:41-66) + set_packet_props_{partial,full}_relativity
+// (modes/classic/packet_propagation.py:255-318) + RPacket.initialize_line_id (packets/radiative_packet.py:96-110) of
+// packet pid: what the ordering pass writes into the packet's StartRecord
+template <bool FR>
+__device__ __forceinline__ StartRecord start_fields(long long pid, long long seed64) {
+    const KParams &P = cP;
+    StartRecord s;
+    s.pid = (int)pid;
+    s.r = P.in_r[pid]; s.mu = P.in_mu[pid]; s.nu = P.in_nu[pid]; s.energy = P.in_energy[pid];
+    const uint2 sx = seed_expand(seed64);
+    s.seed = sx.x; s.x397 = sx.y;
+    double velocity = s.r / P.t_exp;
+    double inv_doppler = inverse_doppler_factor<FR>(velocity, s.mu);
+    if (FR) {
+        double beta = (s.r / P.t_exp) / C_LIGHT;
+        s.nu *= inv_doppler; s.energy *= inv_doppler;
+        s.mu = (s.mu + beta) / (1 + beta * s.mu);
+    } else {
+        s.nu *= inv_doppler; s.energy *= inv_doppler;
+    }
+    // L - searchsorted(nu[::-1], comov_nu, 'left') == #lines with nu_line >= comov_nu
+    double dop = doppler_factor<FR>(velocity, s.mu);
+    int lo = first_line_below(s.nu * dop);
+    if (lo == P.n_lines) lo -= 1;
+    s.next_line = lo;
+    return s;
+}
+
+// the prologue of packet_propagation (modes/classic/packet_propagation.py:99-122) for the packet at processing slot `slot`
 // VP = true: the caller traces virtual packets per lane (classic scan kernel).  VP = false (continuum mode; the jump kernels,
 // which run theirs warp-cooperatively or not at all): that code, and the registers the call to it would clobber, stay out
 // of the kernel
 template <bool FR, bool VP = true>
-__device__ __noinline__ void start_packet_impl(Lane &p, Rng &rng, long long pid, Counters &c) {
+__device__ __noinline__ void start_packet_impl(Lane &p, Rng &rng, long long slot, Counters &c) {
     const KParams &P = cP;
-    const int L = P.n_lines;
-    p.pid = (int)pid;
-    p.r = P.in_r[pid]; p.mu = P.in_mu[pid]; p.nu = P.in_nu[pid]; p.energy = P.in_energy[pid];
-    p.shell = 0; p.status = ST_IN_PROCESS; p.icount = 0; p.bbuf = -1; p.nev = 0; p.nsteps = 0; p.seg_open = 0;
-    rng.start(P.seed[pid], P.seed_x397[pid], (unsigned)pid);
-    // set_packet_props_{partial,full}_relativity, modes/classic/packet_propagation.py:255-318
-    double velocity = p.r / P.t_exp;
-    double inv_doppler = inverse_doppler_factor<FR>(velocity, p.mu);
-    if (FR) {
-        double beta = (p.r / P.t_exp) / C_LIGHT;
-        p.nu *= inv_doppler; p.energy *= inv_doppler;
-        p.mu = (p.mu + beta) / (1 + beta * p.mu);
-    } else {
-        p.nu *= inv_doppler; p.energy *= inv_doppler;
-    }
-    // RPacket.initialize_line_id, packets/radiative_packet.py:96-110:
-    // L - searchsorted(nu[::-1], comov_nu, 'left') == #lines with nu_line >= comov_nu
-    double dop = doppler_factor<FR>(velocity, p.mu);
-    int lo = FR ? first_line_below(p.nu * dop) : first_line_below_call(p.nu * dop);  // (see first_line_below_call)
-    if (lo == L) lo -= 1;
-    p.next_line = lo;
+    const int pid = start_from_record(p, rng, slot);
     if (P.last_type) {  // TrackerLastInteraction.__init__, tracker_last_interaction.py:55-82
         const double qnan = __longlong_as_double(0x7ff8000000000000ll);
         P.last_type[pid] = -1; P.last_event_id[pid] = 0; P.last_shell[pid] = -1;
@@ -1345,9 +1373,9 @@ __device__ __noinline__ void start_packet_impl(Lane &p, Rng &rng, long long pid,
     c.boundary++;
 }
 template <bool FR, bool VP = true>
-__device__ __forceinline__ void start_packet(Lane &p, Rng &rng, long long pid, Counters &c) {
+__device__ __forceinline__ void start_packet(Lane &p, Rng &rng, long long slot, Counters &c) {
     Lane lp; Rng lr = rng; Counters lc;
-    start_packet_impl<FR, VP>(lp, lr, pid, lc);  // sets every field of lp
+    start_packet_impl<FR, VP>(lp, lr, slot, lc);  // sets every field of lp
     p = lp; rng = lr; flush_rare(lc);
 }
 
@@ -1515,8 +1543,8 @@ struct WarpFeed {
         const KParams &P = cP;
         const int lane = threadIdx.x & 31;
         const unsigned freemask = ~busy_mask;
-        // Refill in batches: starting a packet (loads, frame transform, line search, first virtual-packet volley)
-        // is a long scalar detour for the whole warp, so wait until refill_min lanes are free (or the warp is empty).
+        // Refill in batches: starting a packet (the record load, trackers, first virtual-packet volley) is a scalar
+        // detour for the whole warp, so wait until refill_min lanes are free (or the warp is empty).
         if (!exhausted && !(__popc(freemask) >= P.refill_min || freemask == FULL)) return;
         if (done) { finish_packet(p, rng, c); done = false; }
         if (exhausted) return;
@@ -1528,8 +1556,7 @@ struct WarpFeed {
         if (!has) {
             const unsigned long long slot = base + (unsigned long long)__popc(freemask & ((1u << lane) - 1u));
             if (slot < (unsigned long long)P.n_packets) {
-                const long long pid = P.order ? (long long)P.order[slot] : (long long)slot;
-                if (ESCAPE) start_packet_impl<FR, VP>(p, rng, pid, c); else start_packet<FR, VP>(p, rng, pid, c);
+                if (ESCAPE) start_packet_impl<FR, VP>(p, rng, (long long)slot, c); else start_packet<FR, VP>(p, rng, (long long)slot, c);
                 has = true;
             }
         }
@@ -2475,13 +2502,35 @@ __global__ void order_scan_kernel(unsigned *hist, int n_keys) {
         __syncthreads();
     }
 }
-__global__ void order_scatter_kernel(const double *nu, long long n, int shift, long long key_min, int n_keys, unsigned *cursor, int *order) {
+// The pass also writes each packet's StartRecord at its slot (START::at: start_fields of the transport mode), and the seed
+// words by packet id for rng_replay_tier1.  Its reads of the packet arrays stay coalesced (i is sequential per thread); the
+// transport kernel's refills then read consecutive records.
+template <bool FR>
+struct ClassicStart {
+    __device__ __forceinline__ static StartRecord at(long long pid, long long seed64) { return start_fields<FR>(pid, seed64); }
+};
+template <class START>
+__device__ __forceinline__ void write_start(long long i, long long slot, const long long *seeds64, unsigned *seed32, unsigned *x397,
+                                            StartRecord *rec) {
+    const StartRecord s = START::at(i, seeds64[i]);
+    seed32[i] = s.seed; x397[i] = s.x397;
+    rec[slot] = s;
+}
+// sort_packets = 0: packet i at slot i
+template <class START>
+__global__ void start_record_kernel(long long n, const long long *seeds64, unsigned *seed32, unsigned *x397, StartRecord *rec) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) write_start<START>(i, i, seeds64, seed32, x397, rec);
+}
+template <class START>
+__global__ void order_scatter_kernel(const double *nu, long long n, int shift, long long key_min, int n_keys, unsigned *cursor,
+                                     const long long *seeds64, unsigned *seed32, unsigned *x397, StartRecord *rec) {
     __shared__ unsigned sh[ORDER_SMEM_KEYS];  // count of the block per key, then the block's first slot of the key
     const long long base = (long long)blockIdx.x * blockDim.x * ORDER_ITEMS;
     if (n_keys > ORDER_SMEM_KEYS) {  // too many keys for the block's counters: one global atomic per packet
         for (int q = 0; q < ORDER_ITEMS; q++) {
             const long long i = base + (long long)q * blockDim.x + threadIdx.x;
-            if (i < n) order[atomicAdd(&cursor[order_key(nu[i], shift, key_min, n_keys)], 1u)] = (int)i;
+            if (i < n) write_start<START>(i, atomicAdd(&cursor[order_key(nu[i], shift, key_min, n_keys)], 1u), seeds64, seed32, x397, rec);
         }
         return;
     }
@@ -2500,7 +2549,7 @@ __global__ void order_scatter_kernel(const double *nu, long long n, int shift, l
 #pragma unroll
     for (int q = 0; q < ORDER_ITEMS; q++) {
         const long long i = base + (long long)q * blockDim.x + threadIdx.x;
-        if (key[q] >= 0) order[sh[key[q]] + rank[q]] = (int)i;
+        if (key[q] >= 0) write_start<START>(i, sh[key[q]] + rank[q], seeds64, seed32, x397, rec);
     }
 }
 
