@@ -10,6 +10,7 @@
 #include <algorithm>
 
 #include "../../include/tardis_b200.h"
+#include "device_buffer.cuh"
 #include "continuum_bins.cuh"
 #include "continuum_macro_build.cuh"
 #include "transport_kernel.cuh"
@@ -23,34 +24,12 @@
 
 namespace {
 
-thread_local std::string g_last_error;
-
-int fail(int code, const std::string &msg) {
-    g_last_error = msg;
-    return code;
-}
-
 #define CK(call)                                                                                     \
     do {                                                                                             \
         cudaError_t err__ = (call);                                                                  \
         if (err__ != cudaSuccess)                                                                    \
             return fail(TB200_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(err__));      \
     } while (0)
-
-template <typename T> struct DBuf {
-    T *p = nullptr;
-    size_t n = 0;
-    int ensure(size_t count) {
-        if (count <= n && p) return TB200_OK;
-        if (p) cudaFree(p);
-        p = nullptr; n = 0;
-        cudaError_t e = cudaMalloc((void **)&p, (count ? count : 1) * sizeof(T));
-        if (e != cudaSuccess) return fail(TB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-        n = count;
-        return TB200_OK;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
@@ -60,8 +39,9 @@ struct tb200_engine {
     int device = 0;
     int sm_count = 132;
     size_t smem_optin = 227 * 1024;  // largest dynamic + static shared memory one CTA may opt in to (H100: 227 KiB)
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
+    // declared before every buffer, so that the buffers are freed first
+    Stream stream, h2d_stream, d2h_stream;
+    Event ev_start, ev_stop, ev_fin;
     bool have_model = false;
     bool timing_valid = false;
     int64_t launches = 0;
@@ -74,8 +54,6 @@ struct tb200_engine {
     int algorithm = 1;  // 0 = scan (stream the line list), 1 = jump (prefix-table search + range updates; default)
     int vol_min = 24;     // warp-cooperative volleys start when this many lanes of a warp wait for one
     int pooled = 1;     // jump, classic mode: packet pool per warp (transport_pool_kernel); 0 = one packet per lane
-    cudaEvent_t ev_fin = nullptr;
-    cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
     int pipeline_chunks = 8;        // tb200_run splits the packets so that H2D / kernel / D2H overlap
     int pipeline_edges = 1;         // short first and last range (their copies are the exposed ones)
     double nu_typ = 1.0;
@@ -205,16 +183,15 @@ int tb200_create(int device_id, tb200_engine **engine) {
     en->device = device_id;
     cudaDeviceProp prop;
     cudaError_t ce = cudaGetDeviceProperties(&prop, device_id);
-    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&en->stream, cudaStreamNonBlocking);
-    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&en->h2d_stream, cudaStreamNonBlocking);
-    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&en->d2h_stream, cudaStreamNonBlocking);
-    if (ce == cudaSuccess) ce = cudaEventCreate(&en->ev_start);
-    if (ce == cudaSuccess) ce = cudaEventCreate(&en->ev_stop);
-    if (ce == cudaSuccess) ce = cudaEventCreate(&en->ev_fin);
+    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&en->stream.h, cudaStreamNonBlocking);
+    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&en->h2d_stream.h, cudaStreamNonBlocking);
+    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&en->d2h_stream.h, cudaStreamNonBlocking);
+    if (ce == cudaSuccess) ce = cudaEventCreate(&en->ev_start.h);
+    if (ce == cudaSuccess) ce = cudaEventCreate(&en->ev_stop.h);
+    if (ce == cudaSuccess) ce = cudaEventCreate(&en->ev_fin.h);
     if (ce != cudaSuccess) {  // nothing half-built is handed out or left behind
-        const std::string why = std::string("tb200_create: ") + cudaGetErrorString(ce);
-        tb200_destroy(en);
-        return fail(TB200_ERR_CUDA, why);
+        delete en;
+        return fail(TB200_ERR_CUDA, std::string("tb200_create: ") + cudaGetErrorString(ce));
     }
     en->sm_count = prop.multiProcessorCount;
     en->smem_optin = prop.sharedMemPerBlockOptin;
@@ -226,37 +203,7 @@ void tb200_destroy(tb200_engine *en) {
     if (!en) return;
     cudaSetDevice(en->device);
     cudaStreamSynchronize(en->stream);
-    en->r_inner.release(); en->r_outer.release(); en->n_e.release(); en->nu_line.release(); en->tau_t.release();
-    en->prefix.release(); en->first_le.release(); en->diff.release(); en->xfer.release(); en->bulk_rep.release(); en->cnt_rep.release(); en->macro_guide.release(); en->macro_next.release(); en->macro_entry.release(); en->tp_t.release(); en->grid.release(); en->staging.release();
-    en->t_e.release(); en->bf_thr.release(); en->pi_min.release(); en->pi_max.release(); en->x_sect.release(); en->phot_nus.release();
-    en->cb_B.release(); en->cb_mom.release(); en->cont_lit.release(); en->cb_guide.release(); en->cb_nact.release(); en->cb_pos.release(); en->cb_chi_lin.release();
-    en->cb_act_start.release(); en->cb_act.release();
-    en->ff_factor.release(); en->chi_bf_t.release(); en->emiss_t.release(); en->markov_cum.release(); en->pi_refs.release(); en->pi_act.release();
-    en->mk_p_t.release(); en->mk_q.release(); en->mk_r.release(); en->mk_c.release(); en->mk_keep.release();
-    en->mk_type.release(); en->mk_dest.release(); en->mk_err.release();
-    en->ct_off.release(); en->ct_energy.release(); en->ct_tab.release(); en->ct_shell.release(); en->op_cont_tp_t.release();
-    en->line2macro.release(); en->block_edge.release(); en->ttype.release(); en->dest.release(); en->tline.release();
-    en->est.release(); en->in_r.release(); en->in_nu.release(); en->in_mu.release(); en->in_energy.release();
-    en->out_nu.release(); en->out_energy.release(); en->seeds64.release(); en->seed32.release(); en->x397.release(); en->ps_l_array.release(); en->ps_rejected.release(); en->ps_count.release();
-    en->start_rec.release(); en->order_hist.release();
-    en->at_lower.release(); en->at_upper.release(); en->at_meta.release(); en->at_nlte.release(); en->at_g.release(); en->at_wfl.release();
-    en->at_flu.release(); en->at_ful.release(); en->at_elo.release(); en->at_eup.release(); en->op_lnd.release(); en->op_beta_t.release();
-    en->op_stim_t.release(); en->op_tp_norm_t.release(); en->op_dvdr.release();
-    en->sf_lvl_ptr.release(); en->sf_lvl_lines.release(); en->sf_in_ptr.release(); en->sf_in_rows.release(); en->sf_in_src.release(); en->sf_em_row.release();
-    en->fi_cells.release(); en->fi_shells.release(); en->fi_weights.release(); en->fi_freq.release(); en->fi_I.release(); en->fi_L.release();
-    en->fi_att_t.release(); en->fi_jred_t.release(); en->fi_jblue_t.release();
-    en->sf_upper.release(); en->sf_wave.release(); en->sf_norm.release(); en->sf_e.release(); en->sf_c0.release(); en->sf_c1.release(); en->sf_att_t.release();
-    en->sf_jred_t.release(); en->sf_jblue_t.release(); en->sf_in_t.release(); en->sf_in2_t.release(); en->sf_delta.release();
-    en->rf_shell.release(); en->rf_volume.release(); en->rf_jblues_t.release(); en->rf_in_t.release();
-    en->rng_buf.release(); en->ctrl.release(); en->error.release(); en->last_i.release(); en->last_d.release();
-    en->events.release(); en->event_counts.release(); en->vlog_d.release(); en->vlog_pid.release();
-    if (en->ev_start) cudaEventDestroy(en->ev_start);
-    if (en->ev_stop) cudaEventDestroy(en->ev_stop);
-    if (en->ev_fin) cudaEventDestroy(en->ev_fin);
-    if (en->h2d_stream) cudaStreamDestroy(en->h2d_stream);
-    if (en->d2h_stream) cudaStreamDestroy(en->d2h_stream);
-    if (en->stream) cudaStreamDestroy(en->stream);
-    delete en;
+    delete en;  // the buffers, then the events and streams (tb200_engine's owners)
 }
 
 int tb200_set_option(tb200_engine *en, const char *name, int64_t value) {
@@ -297,6 +244,19 @@ static int upload_strided_table(tb200_engine *en, const double *src, int64_t row
                                                                                         (int)rows, (int)shells, pad, dst.p);
     en->launches++;
     CK(cudaGetLastError());
+    return TB200_OK;
+}
+
+// The way back: rows x S of a shell-major [S][pad] table to the host as [rows][S] (line-major), through staging.  Only
+// queued on en->stream: the caller synchronises before it reads dst.
+static int download_line_major(tb200_engine *en, const double *src_t, int rows, int pad, double *dst) {
+    const long long cells = (long long)rows * en->S;
+    int r;
+    if ((r = en->staging.ensure((size_t)cells))) return r;
+    tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, en->stream>>>(src_t, rows, en->S, pad, en->staging.p);
+    en->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(dst, en->staging.p, (size_t)cells * sizeof(double), cudaMemcpyDeviceToHost, en->stream));
     return TB200_OK;
 }
 
@@ -597,6 +557,16 @@ static void set_typical_energy(tb200_engine *en, const tb200_packets *pk) {
     else if (pk->n_packets > 0) en->e_typ = typical_energy(pk->initial_energies, pk->n_packets);
 }
 
+// The per-packet arrays of the transport, for n packets.
+static int ensure_packet_arrays(tb200_engine *en, int64_t n) {
+    int r;
+    if ((r = en->in_r.ensure(n)) || (r = en->in_nu.ensure(n)) || (r = en->in_mu.ensure(n)) || (r = en->in_energy.ensure(n)) ||
+        (r = en->out_nu.ensure(n)) || (r = en->out_energy.ensure(n)) || (r = en->seeds64.ensure(n)) || (r = en->seed32.ensure(n)) ||
+        (r = en->x397.ensure(n)))
+        return r;
+    return TB200_OK;
+}
+
 int tb200_upload_packets(tb200_engine *en, const tb200_packets *pk) {
     if (!en || !pk) return fail(TB200_ERR_INVALID, "bad argument");
     if (pk->n_packets < 0 || pk->n_packets > 2000000000LL) return fail(TB200_ERR_INVALID, "n_packets out of range");
@@ -604,10 +574,7 @@ int tb200_upload_packets(tb200_engine *en, const tb200_packets *pk) {
     const int64_t n = pk->n_packets;
     en->N = n;
     int r;
-    if ((r = en->in_r.ensure(n)) || (r = en->in_nu.ensure(n)) || (r = en->in_mu.ensure(n)) || (r = en->in_energy.ensure(n)) ||
-        (r = en->out_nu.ensure(n)) || (r = en->out_energy.ensure(n)) || (r = en->seeds64.ensure(n)) || (r = en->seed32.ensure(n)) ||
-        (r = en->x397.ensure(n)))
-        return r;
+    if ((r = ensure_packet_arrays(en, n))) return r;
     set_typical_energy(en, pk);
     if (n == 0) return TB200_OK;
     CK(cudaMemcpyAsync(en->in_r.p, pk->initial_radii, n * sizeof(double), cudaMemcpyHostToDevice, en->stream));
@@ -662,9 +629,7 @@ static int create_packets_range(tb200_engine *en, const tb200_packet_source *src
     const int64_t n = src->n_packets, count = hi - lo;
     en->N = count;
     int r;
-    if ((r = en->in_r.ensure(count)) || (r = en->in_nu.ensure(count)) || (r = en->in_mu.ensure(count)) || (r = en->in_energy.ensure(count)) ||
-        (r = en->out_nu.ensure(count)) || (r = en->out_energy.ensure(count)) || (r = en->seeds64.ensure(count)) || (r = en->seed32.ensure(count)) ||
-        (r = en->x397.ensure(count)) || (r = en->ps_l_array.ensure((size_t)src->n_l)) || (r = en->ps_rejected.ensure(PS_MAX_REJECTED)) ||
+    if ((r = ensure_packet_arrays(en, count)) || (r = en->ps_l_array.ensure((size_t)src->n_l)) || (r = en->ps_rejected.ensure(PS_MAX_REJECTED)) ||
         (r = en->ps_count.ensure(2)))
         return r;
     if (n == 0) return TB200_OK;
@@ -1104,20 +1069,9 @@ int tb200_download(tb200_engine *en, tb200_outputs *o) {
     } else if (en->continuum && o->ff_heating_estimator) {
         CK(cudaMemcpyAsync(o->ff_heating_estimator, en->est.p + en->off_ffheat, S * sizeof(double), cudaMemcpyDeviceToHost, st));
     }
-    if (o->j_blue || o->edotlu) {
-        int r;
-        if ((r = en->staging.ensure((size_t)L * S))) return r;
-        const long long total = (long long)L * S;
-        double *dsts[2] = {o->j_blue, o->edotlu};
-        size_t offs[2] = {en->off_jblue, en->off_edotlu};
-        for (int k = 0; k < 2; k++) {
-            if (!dsts[k]) continue;
-            tb::transpose_to_line_major<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(en->est.p + offs[k], L, S, en->lpad, en->staging.p);
-            en->launches++;
-            CK(cudaGetLastError());
-            CK(cudaMemcpyAsync(dsts[k], en->staging.p, total * sizeof(double), cudaMemcpyDeviceToHost, st));
-        }
-    }
+    int r;
+    if (o->j_blue && (r = download_line_major(en, en->est.p + en->off_jblue, L, en->lpad, o->j_blue))) return r;
+    if (o->edotlu && (r = download_line_major(en, en->est.p + en->off_edotlu, L, en->lpad, o->edotlu))) return r;
     if (o->last_interaction_type && en->track_last && N) {
         long long *li = en->last_i.p; double *ld = en->last_d.p;
         int64_t *di[5] = {o->last_interaction_type, o->last_event_id, o->last_shell_id, o->last_line_absorb_id, o->last_line_emit_id};
@@ -1181,15 +1135,12 @@ static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_output
     CK(cudaSetDevice(en->device));
     if (pk) {
         en->N = n;
-        if ((r = en->in_r.ensure(n)) || (r = en->in_nu.ensure(n)) || (r = en->in_mu.ensure(n)) || (r = en->in_energy.ensure(n)) ||
-            (r = en->out_nu.ensure(n)) || (r = en->out_energy.ensure(n)) || (r = en->seeds64.ensure(n)) || (r = en->seed32.ensure(n)) ||
-            (r = en->x397.ensure(n)))
-            return r;
+        if ((r = ensure_packet_arrays(en, n))) return r;
     }
     if ((r = prepare_tracking(en, nullptr))) return r;
     if (pk) set_typical_energy(en, pk);
-    std::vector<cudaEvent_t> ev_up(chunks), ev_k0(chunks), ev_k1(chunks);
-    for (int c = 0; c < chunks; c++) { CK(cudaEventCreateWithFlags(&ev_up[c], cudaEventDisableTiming)); CK(cudaEventCreate(&ev_k0[c])); CK(cudaEventCreate(&ev_k1[c])); }
+    std::vector<Event> ev_up(chunks), ev_k0(chunks), ev_k1(chunks);
+    for (int c = 0; c < chunks; c++) { CK(cudaEventCreateWithFlags(&ev_up[c].h, cudaEventDisableTiming)); CK(cudaEventCreate(&ev_k0[c].h)); CK(cudaEventCreate(&ev_k1[c].h)); }
     int rc = TB200_OK;
     // Range boundaries: the first and the last range are a quarter of the others -- the H2D copy of the first range and the
     // D2H copy of the last one are the only transfers nothing hides (option pipeline_edges = 0: all ranges equal)
@@ -1234,7 +1185,6 @@ static int run_pipelined(tb200_engine *en, const tb200_packets *pk, tb200_output
     for (int c = 0; c < chunks; c++) {
         float f = 0.0f;
         if (rc == TB200_OK && cudaEventElapsedTime(&f, ev_k0[c], ev_k1[c]) == cudaSuccess) total_ms += f;
-        cudaEventDestroy(ev_up[c]); cudaEventDestroy(ev_k0[c]); cudaEventDestroy(ev_k1[c]);
     }
     if (rc) return rc;
     en->chunk_kernel_ms = total_ms; en->chunked_timing = true; en->timing_valid = true;
@@ -1258,11 +1208,17 @@ int tb200_run_resident(tb200_engine *en, tb200_outputs *o) {
     return run_pipelined(en, nullptr, o);
 }
 
-int tb200_line_accumulators(tb200_engine *en, void **device_ptr, int64_t *n_words, double *scale_j_blue, double *scale_edotlu) {
-    if (!en || !device_ptr || !n_words || !scale_j_blue || !scale_edotlu) return fail(TB200_ERR_INVALID, "bad argument");
+static int check_line_accumulators(const tb200_engine *en) {
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if (en->algorithm != 1 || en->nonhomologous || !en->diff.p)
         return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump), outside the nonhomologous mode");
+    return TB200_OK;
+}
+
+int tb200_line_accumulators(tb200_engine *en, void **device_ptr, int64_t *n_words, double *scale_j_blue, double *scale_edotlu) {
+    if (!en || !device_ptr || !n_words || !scale_j_blue || !scale_edotlu) return fail(TB200_ERR_INVALID, "bad argument");
+    int r;
+    if ((r = check_line_accumulators(en))) return r;
     *device_ptr = en->diff.p;
     *n_words = (int64_t)en->S * (en->lpad + 1) * 4;
     *scale_j_blue = en->diff_scale2; *scale_edotlu = en->diff_scale1;  // scale1: w1 -> Edotlu, scale2: w2 -> J_blue
@@ -1271,9 +1227,8 @@ int tb200_line_accumulators(tb200_engine *en, void **device_ptr, int64_t *n_word
 
 int tb200_finalize_line_estimators(tb200_engine *en) {
     if (!en) return fail(TB200_ERR_INVALID, "bad argument");
-    if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
-    if (en->algorithm != 1 || en->nonhomologous || !en->diff.p)
-        return fail(TB200_ERR_INVALID, "the line accumulators exist only with algorithm = 1 (jump), outside the nonhomologous mode");
+    int r;
+    if ((r = check_line_accumulators(en))) return r;
     if (en->diff_scale1 == 0.0 || en->diff_scale2 == 0.0) return fail(TB200_ERR_INVALID, "no transport has filled the line accumulators yet");
     CK(cudaSetDevice(en->device));
     const int full_rel = (en->cfg.enable_full_relativity || en->continuum) ? 1 : 0;
@@ -1355,14 +1310,7 @@ int tb200_solve_radiation_field(tb200_engine *en, const tb200_radfield_params *p
     CK(cudaGetLastError());
     if (t_radiative) CK(cudaMemcpyAsync(t_radiative, en->rf_shell.p, S * sizeof(double), cudaMemcpyDeviceToHost, st));
     if (dilution_factor) CK(cudaMemcpyAsync(dilution_factor, en->rf_shell.p + S, S * sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (j_blues) {
-        if ((r = en->staging.ensure((size_t)L * S))) return r;
-        const long long cells = (long long)L * S;
-        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(en->rf_jblues_t.p, L, S, lpad, en->staging.p);
-        en->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(j_blues, en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
-    }
+    if (j_blues && (r = download_line_major(en, en->rf_jblues_t.p, L, lpad, j_blues))) return r;
     CK(cudaStreamSynchronize(st));
     en->rf_valid = true;
     return TB200_OK;
@@ -1540,14 +1488,9 @@ int tb200_solve_source_function(tb200_engine *en, const tb200_source_function_pa
     CK(cudaGetLastError());
     double *outs[3] = {att_S_ul, Jred_lu, Jblue_lu};
     const double *srcs[3] = {en->sf_att_t.p, en->sf_jred_t.p, en->sf_jblue_t.p};
-    const long long cells = (long long)L * S;
     for (int k = 0; k < 3; k++) {
         if (!outs[k]) continue;
-        if ((r = en->staging.ensure((size_t)cells))) return r;
-        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(srcs[k], L, S, lpad, en->staging.p);
-        en->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(outs[k], en->staging.p, (size_t)cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+        if ((r = download_line_major(en, srcs[k], L, lpad, outs[k]))) return r;
         CK(cudaStreamSynchronize(st));  // staging is reused
     }
     if (e_dot_u) {  // [n_levels, S] C-order on the host; on the device it lies [S][n_levels]
@@ -1673,12 +1616,9 @@ int tb200_formal_integral(tb200_engine *en, const tb200_formal_integral_params *
         if ((r = upload_strided_table(en, p->Jblue_lu, L, S, S, 1, lpad, en->fi_jblue_t))) return r;
         T.att_t = en->fi_att_t.p; T.jred_t = en->fi_jred_t.p; T.jblue_t = en->fi_jblue_t.p;
     }
-    cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr;
-    auto drop = [&]() { if (e0) cudaEventDestroy(e0); if (e1) cudaEventDestroy(e1); if (e2) cudaEventDestroy(e2); };
-    if (cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess || cudaEventCreate(&e2) != cudaSuccess) {
-        drop();
+    Event e0, e1, e2;
+    if (cudaEventCreate(&e0.h) != cudaSuccess || cudaEventCreate(&e1.h) != cudaSuccess || cudaEventCreate(&e2.h) != cudaSuccess)
         return fail(TB200_ERR_CUDA, "cudaEventCreate failed");
-    }
     tbfi::Cell *cells = reinterpret_cast<tbfi::Cell *>(en->fi_cells.p);
     cudaEventRecord(e0, st);
     fi_cells_kernel<<<(unsigned)((n_cells + 255) / 256), 256, 0, st>>>(T, reinterpret_cast<const tbfi::ShellWeights *>(en->fi_weights.p), S2, cells);
@@ -1686,10 +1626,10 @@ int tb200_formal_integral(tb200_engine *en, const tb200_formal_integral_params *
     cudaEventRecord(e1, st);
     if (n_frequencies > 0) {
         cudaError_t cf = cudaMemcpyAsync(en->fi_freq.p, frequencies, (size_t)n_frequencies * sizeof(double), cudaMemcpyHostToDevice, st);
-        if (cf != cudaSuccess) { drop(); return fail(TB200_ERR_CUDA, std::string("cudaMemcpyAsync(frequencies): ") + cudaGetErrorString(cf)); }
+        if (cf != cudaSuccess) return fail(TB200_ERR_CUDA, std::string("cudaMemcpyAsync(frequencies): ") + cudaGetErrorString(cf));
         const int n_blocks = (P - 1 + 31) / 32;  // impact parameters 1 ... P - 1
         const long long items = (long long)n_frequencies * n_blocks;
-        if ((items + FI_WARPS - 1) / FI_WARPS > 2147483647LL) { drop(); return fail(TB200_ERR_INVALID, "n_frequencies x n_impact_parameters too large for one launch"); }
+        if ((items + FI_WARPS - 1) / FI_WARPS > 2147483647LL) return fail(TB200_ERR_INVALID, "n_frequencies x n_impact_parameters too large for one launch");
         tbfi::Shells g{en->fi_shells.p, en->fi_shells.p + S2, en->fi_shells.p + 2 * (size_t)S2, S2, 1 / en->t_exp, en->t_exp / tbfi::C_INV};
         fi_rays_kernel<<<(unsigned)((items + FI_WARPS - 1) / FI_WARPS), FI_WARPS * 32, 0, st>>>(g, en->nu_line.p, L, cells, en->fi_freq.p, (int)n_frequencies, P,
                                                                                               n_blocks, p->inner_temperature, en->fi_I.p);
@@ -1698,17 +1638,16 @@ int tb200_formal_integral(tb200_engine *en, const tb200_formal_integral_params *
     }
     cudaEventRecord(e2, st);
     cudaError_t ce = cudaGetLastError();
-    if (ce != cudaSuccess) { drop(); return fail(TB200_ERR_CUDA, cudaGetErrorString(ce)); }
+    if (ce != cudaSuccess) return fail(TB200_ERR_CUDA, cudaGetErrorString(ce));
     if (n_frequencies > 0) {
         cudaMemcpyAsync(luminosity_densities, en->fi_L.p, (size_t)n_frequencies * sizeof(double), cudaMemcpyDeviceToHost, st);
         if (intensities_nu_p) cudaMemcpyAsync(intensities_nu_p, en->fi_I.p, (size_t)n_frequencies * P * sizeof(double), cudaMemcpyDeviceToHost, st);
     }
     ce = cudaStreamSynchronize(st);
-    if (ce != cudaSuccess) { drop(); return fail(TB200_ERR_CUDA, cudaGetErrorString(ce)); }
+    if (ce != cudaSuccess) return fail(TB200_ERR_CUDA, cudaGetErrorString(ce));
     float a = 0.0f, b = 0.0f;
     cudaEventElapsedTime(&a, e0, e1); cudaEventElapsedTime(&b, e1, e2);
     en->fi_cells_ms = a; en->fi_rays_ms = b;
-    drop();
     return TB200_OK;
 }
 
@@ -1910,6 +1849,15 @@ int tb200_set_atomic_data(tb200_engine *en, const tb200_atomic_data *a) {
     return TB200_OK;
 }
 
+// Waits for tb200_build_opacity's kernels and reports a non-finite tau_sobolev they flagged in the error word.
+static int wait_opacity_build(tb200_engine *en) {
+    CK(cudaStreamSynchronize(en->stream));
+    int err = 0;
+    CK(cudaMemcpy(&err, en->error.p, sizeof(int), cudaMemcpyDeviceToHost));
+    if (err == tb::ERR_OPACITY) return fail(TB200_ERR_INVALID, "Some tau_sobolevs are nan, inf, -inf in tau_sobolevs. Something went wrong!");
+    return TB200_OK;
+}
+
 int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
     // continuum rates with beta / stim: the line rows read the caller's tables, tau is the model's (not rebuilt)
     const bool host_lines = p && p->continuum && (p->continuum->beta_sobolev || p->continuum->stimulated_emission_factor);
@@ -1992,10 +1940,7 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
                 if ((r = en->op_cont_tp_t.ensure((size_t)S * en->tpad))) return r;
                 CK(cudaMemcpyAsync(en->op_cont_tp_t.p, en->mk_p_t.p, (size_t)S * en->tpad * sizeof(double), cudaMemcpyDeviceToDevice, st));
             }
-            CK(cudaStreamSynchronize(st));
-            int err = 0;
-            CK(cudaMemcpy(&err, en->error.p, sizeof(int), cudaMemcpyDeviceToHost));
-            if (err == tb::ERR_OPACITY) return fail(TB200_ERR_INVALID, "Some tau_sobolevs are nan, inf, -inf in tau_sobolevs. Something went wrong!");
+            if ((r = wait_opacity_build(en))) return r;
             // the chain is built from this table next (tb200_build_absorbing_markov with transition_probabilities == NULL),
             // which also finishes the tables the kernels read
             en->op_cont_valid = en->keep_opacity_tables != 0;
@@ -2015,11 +1960,7 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
             CK(cudaMemcpyAsync(en->op_tp_norm_t.p, en->tp_t.p, (size_t)S * en->tpad * sizeof(double), cudaMemcpyDeviceToDevice, st));
         }
     }
-    if ((r = finish_opacity_tables(en))) return r;
-    CK(cudaStreamSynchronize(st));
-    int err = 0;
-    CK(cudaMemcpy(&err, en->error.p, sizeof(int), cudaMemcpyDeviceToHost));
-    if (err == tb::ERR_OPACITY) return fail(TB200_ERR_INVALID, "Some tau_sobolevs are nan, inf, -inf in tau_sobolevs. Something went wrong!");
+    if ((r = finish_opacity_tables(en)) || (r = wait_opacity_build(en))) return r;
     en->opacity_pending = false;
     return TB200_OK;
 }
@@ -2028,7 +1969,6 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
     if (!en) return fail(TB200_ERR_INVALID, "bad argument");
     if (!en->have_model || en->opacity_pending) return fail(TB200_ERR_NO_MODEL, "no opacity tables on the device");
     CK(cudaSetDevice(en->device));
-    const int S = en->S, L = en->L;
     cudaStream_t st = en->stream;
     int r;
     double *dst[3] = {tau, beta, stim};
@@ -2036,12 +1976,7 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
     for (int k = 0; k < 3; k++) {
         if (!dst[k]) continue;
         if (!src[k]) return fail(TB200_ERR_INVALID, "this table was not built on the device");
-        if ((r = en->staging.ensure((size_t)L * S))) return r;
-        const long long cells = (long long)L * S;
-        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(src[k], L, S, en->lpad, en->staging.p);
-        en->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(dst[k], en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+        if ((r = download_line_major(en, src[k], en->L, en->lpad, dst[k]))) return r;
         CK(cudaStreamSynchronize(st));
     }
     if (tp) {
@@ -2050,12 +1985,7 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
                                            "keep_opacity_tables before it; the deactivation table is tb200_download_absorbing_markov's)");
         const double *kept = en->continuum ? en->op_cont_tp_t.p : en->op_tp_norm_t.p;
         if (!en->have_macro || !kept) return fail(TB200_ERR_INVALID, "transition_probabilities: set the option keep_opacity_tables before tb200_build_opacity");
-        if ((r = en->staging.ensure((size_t)en->T * S))) return r;
-        const long long cells = (long long)en->T * S;
-        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(kept, en->T, S, en->tpad, en->staging.p);
-        en->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(tp, en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+        if ((r = download_line_major(en, kept, en->T, en->tpad, tp))) return r;
         CK(cudaStreamSynchronize(st));
     }
     return TB200_OK;
@@ -2205,15 +2135,8 @@ int tb200_download_absorbing_markov(tb200_engine *en, double *matrix, double *de
         const size_t nm = (size_t)S * en->mk_keep_n * en->mk_keep_n;
         CK(cudaMemcpyAsync(matrix, en->mk_keep.p, nm * sizeof(double), cudaMemcpyDeviceToHost, st));
     }
-    if (deactivating) {
-        int r;
-        if ((r = en->staging.ensure((size_t)en->T * S))) return r;
-        const long long cells = (long long)en->T * S;
-        tb::transpose_to_line_major<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(en->op_tp_norm_t.p, en->T, S, en->tpad, en->staging.p);
-        en->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(deactivating, en->staging.p, cells * sizeof(double), cudaMemcpyDeviceToHost, st));
-    }
+    int r;
+    if (deactivating && (r = download_line_major(en, en->op_tp_norm_t.p, en->T, en->tpad, deactivating))) return r;
     CK(cudaStreamSynchronize(st));
     return TB200_OK;
 }

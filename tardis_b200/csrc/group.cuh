@@ -320,7 +320,7 @@ void tb200_group_destroy(tb200_group *g) {
     for (size_t i = 0; i < g->m.size(); i++) {
         if (i < g->staging.size()) {
             cudaSetDevice(g->m[i]->device);
-            g->staging[i].release();
+            g->staging[i].release();  // here, with its device current: its destructor would run on whichever device is
         }
         tb200_destroy(g->m[i]);
     }
