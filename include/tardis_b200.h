@@ -209,6 +209,14 @@ typedef struct {
      * 1 / N * (2 beta + 1) / (1 - beta^2) / gamma.  relativistic = 0: the plain source, beta ignored. */
     int32_t relativistic;
     double beta;
+    /* BlackBodyWeightedSource (packet_source/black_body_weighted.py:9-108): the stream after the seeds is 5 N doubles for
+     * Carter-Cashwell nus that only give their min and max, then nus = rng.uniform(min, max, N) (= min + (max - min) *
+     * rng.random()), then mus = sqrt(rng.random(N)); energies = I / I.sum() with I = intensity_black_body(nus, T)
+     * (util/base.py:279-302) and the sum in numpy's pairwise order.  Seeds, radii and mus are bit-identical to numpy's;
+     * nus and energies differ from numpy's by the ulps of log, pow and exp (INTEGRATION.md gives the measured bounds).
+     * Refused together with relativistic (the reference has no such source) and for n_packets = 0 (numpy raises on the
+     * zero-size min).  weighted = 0: the sources above. */
+    int32_t weighted;
 } tb200_packet_source;
 int tb200_create_packets(tb200_engine *engine, const tb200_packet_source *source);
 /* resident input arrays -> host (diagnostics / tests / callers that want the PacketCollection); any pointer may be NULL */

@@ -82,10 +82,11 @@ class Config(C.Structure):
 
 
 class PacketSource(C.Structure):
-    """tb200_packet_source (device-side BlackBodySimpleSource)"""
+    """tb200_packet_source (device-side BlackBodySimpleSource, ...Relativistic and BlackBodyWeightedSource)"""
     _fields_ = [
         ("n_packets", C.c_int64), ("seed", C.c_uint64), ("radius", C.c_double), ("temperature", C.c_double),
         ("l_array", _pd), ("n_l", C.c_int64), ("max_seed_val", C.c_uint32), ("relativistic", C.c_int32), ("beta", C.c_double),
+        ("weighted", C.c_int32),
     ]
 
 

@@ -121,6 +121,8 @@ struct tb200_engine {
     DBuf<double> ps_l_array;                 // device-side packet source: l_array, rejected raw draws, {count, overflow}
     DBuf<unsigned long long> ps_rejected;
     DBuf<unsigned> ps_count;
+    DBuf<unsigned long long> ps_minmax;      // weighted source: {min, max} of the Carter-Cashwell nus (as bit patterns)
+    DBuf<double> ps_leaf_sums;               // weighted source: the pairwise-sum leaves that start in this engine's range
     DBuf<unsigned> seed32, x397, order_hist;
     DBuf<tb::StartRecord> start_rec;         // by processing slot (tb::StartRecord), written by the ordering pass
     // radiation-field solve (radfield.cuh): resident results + scratch for host-supplied estimators
@@ -616,15 +618,53 @@ __global__ void packet_source_fill_kernel(tbps::SourceParams P, unsigned long lo
     const unsigned long long i1 = (i0 + PS_CHUNK < hi) ? i0 + PS_CHUNK : hi;
     tbps::fill_chunk(P, i0, i1, r, nu, mu, e, seeds, lo);
 }
+
+// Weighted source, pass 1: min and max of the Carter-Cashwell nus of packets [lo, hi).  nu > 0, so the order of the
+// bit patterns is the order of the values and the reduction is exact in any order.
+__global__ void packet_source_minmax_kernel(tbps::SourceParams P, unsigned long long lo, unsigned long long hi, unsigned long long *mm) {
+    const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned long long i0 = lo + t * PS_CHUNK;
+    double mn = __longlong_as_double(0x7FF0000000000000LL), mx = 0.0;
+    if (i0 < hi) tbps::blackbody_nu_minmax(P, i0, (i0 + PS_CHUNK < hi) ? i0 + PS_CHUNK : hi, mn, mx);
+    for (int o = 16; o > 0; o >>= 1) {
+        mn = fmin(mn, __shfl_xor_sync(0xFFFFFFFFu, mn, o));
+        mx = fmax(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, o));
+    }
+    if ((threadIdx.x & 31) == 0 && mx > 0.0) {
+        atomicMin(mm, (unsigned long long)__double_as_longlong(mn));
+        atomicMax(mm + 1, (unsigned long long)__double_as_longlong(mx));
+    }
+}
+
+// Weighted source, pass 2: thread t takes the pairwise-sum leaves that start in [lo + t PS_CHUNK, ...) (thread 0 also the
+// leaf holding packet lo), stores its packets with I(nu) as their energy and each leaf's sum at its slot.
+__global__ void packet_source_weighted_fill_kernel(tbps::SourceParams P, tbps::WeightedParams W, unsigned long long lo, unsigned long long hi,
+                                                   double *r, double *nu, double *mu, double *e, long long *seeds, double *slots) {
+    const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned long long a = lo + t * PS_CHUNK;
+    if (a >= hi) return;
+    const unsigned long long b = (a + PS_CHUNK < hi) ? a + PS_CHUNK : hi;
+    tbps::weighted_fill_leaves(P, W, a, b, lo, hi, r, nu, mu, e, seeds, slots, tbps::pw_slot(lo));
+}
+
+// Weighted source, pass 3: energy = I / sum, a division as numpy's `intensity / intensity.sum()`.
+__global__ void packet_source_normalize_kernel(double *e, long long n, double sum) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += stride) e[k] = e[k] / sum;
+}
 }  // namespace
 
-// Packets [lo, hi) of the source's n_packets become the engine's resident packets 0 .. hi - lo - 1, bit for bit what
-// the whole set holds there (an engine group generates each member's range in place).
-static int create_packets_range(tb200_engine *en, const tb200_packet_source *src, int64_t lo, int64_t hi) {
+// Everything create_packets_range needs before its kernels: argument checks, the engine's arrays, the rejected draws of
+// the seed segment and the generator parameters.  *ready = false: nothing to generate (no packets, or none in [lo, hi)).
+static int packet_source_setup(tb200_engine *en, const tb200_packet_source *src, int64_t lo, int64_t hi, tbps::SourceParams &P, bool *ready) {
+    *ready = false;
     if (!en || !src) return fail(TB200_ERR_INVALID, "bad argument");
     if (src->n_packets < 0 || src->n_packets > 2000000000LL) return fail(TB200_ERR_INVALID, "n_packets out of range");
     if (!src->l_array || src->n_l < 1 || src->n_l > (1 << 24)) return fail(TB200_ERR_INVALID, "l_array missing");
     if (!(src->temperature > 0) || !(src->radius > 0)) return fail(TB200_ERR_INVALID, "temperature and radius must be positive");
+    if (src->weighted && src->relativistic) return fail(TB200_ERR_INVALID, "the weighted source has no relativistic variant");
+    if (src->weighted && src->n_packets == 0)
+        return fail(TB200_ERR_INVALID, "the weighted source needs at least one packet (the min / max of zero frequencies is undefined)");
     CK(cudaSetDevice(en->device));
     const int64_t n = src->n_packets, count = hi - lo;
     en->N = count;
@@ -636,7 +676,6 @@ static int create_packets_range(tb200_engine *en, const tb200_packet_source *src
     en->e_typ = 1.0 / (double)n;
     CK(cudaMemcpyAsync(en->ps_l_array.p, src->l_array, (size_t)src->n_l * sizeof(double), cudaMemcpyHostToDevice, en->stream));
 
-    tbps::SourceParams P;
     P.origin = tbps::pcg64_from_seed(src->seed);
     P.n = (uint64_t)n;
     const uint32_t pop = src->max_seed_val ? src->max_seed_val : 0xFFFFFFFFu;  // rng.choice(pop, N): integers in [0, pop)
@@ -681,19 +720,124 @@ static int create_packets_range(tb200_engine *en, const tb200_packet_source *src
         P.energy = 1.0 / (double)n * factor / gamma;
     }
     en->e_typ = P.energy;
-    if (count == 0) return TB200_OK;
-    {
-        const unsigned long long threads = ((unsigned long long)count + PS_CHUNK - 1) / PS_CHUNK;
-        packet_source_fill_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, en->stream>>>(P, (unsigned long long)lo, (unsigned long long)hi,
-                                                                                             en->in_r.p, en->in_nu.p, en->in_mu.p, en->in_energy.p,
-                                                                                             en->seeds64.p);
-        en->launches++;
-        CK(cudaGetLastError());
-    }
+    *ready = count > 0;
     return TB200_OK;
 }
 
+// Packets [lo, hi) of the source's n_packets become the engine's resident packets 0 .. hi - lo - 1, bit for bit what
+// the whole set holds there (an engine group generates each member's range in place).  Not the weighted source, whose
+// energies need sums over the whole set: create_weighted_packets.
+static int create_packets_range(tb200_engine *en, const tb200_packet_source *src, int64_t lo, int64_t hi) {
+    tbps::SourceParams P;
+    bool ready;
+    const int r = packet_source_setup(en, src, lo, hi, P, &ready);
+    if (r || !ready) return r;
+    const unsigned long long threads = ((unsigned long long)(hi - lo) + PS_CHUNK - 1) / PS_CHUNK;
+    packet_source_fill_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, en->stream>>>(P, (unsigned long long)lo, (unsigned long long)hi,
+                                                                                         en->in_r.p, en->in_nu.p, en->in_mu.p, en->in_energy.p,
+                                                                                         en->seeds64.p);
+    en->launches++;
+    CK(cudaGetLastError());
+    return TB200_OK;
+}
+
+// The weighted source on members m[0 .. G) holding packets [b[i], b[i + 1]) (one engine: G = 1).  each(f) runs f(i) for
+// every member and returns the first error.  Three passes, with the host between them:
+//   1. every member: min / max of the Carter-Cashwell nus of its range; the host takes the min / max over members;
+//   2. every member: its packets with I(nu) as energy, and the sums of the pairwise-sum leaves that START in its range (a
+//      leaf that runs past the range's end is generated to its end, its packets there not stored); the host combines
+//      all leaf sums along numpy's tree, so the sum does not depend on the number of members;
+//   3. every member: energy = I / sum.
+// Every member's e_typ is the whole set's mean energy, 1 / N.
+extern "C++" {  // a template, inside the C-ABI block
+template <class Each>
+static int create_weighted_packets(const tb200_packet_source *src, tb200_engine *const *m, const int64_t *b, int G, Each each) {
+    std::vector<tbps::SourceParams> P((size_t)G);
+    std::vector<char> ready((size_t)G, 0);
+    std::vector<double> mn((size_t)G, 0.0), mx((size_t)G, 0.0);
+    int r = each([&](int i) -> int {
+        tb200_engine *en = m[i];
+        bool rd;
+        int rr = packet_source_setup(en, src, b[i], b[i + 1], P[(size_t)i], &rd);
+        if (rr || !rd) return rr;
+        ready[(size_t)i] = 1;
+        en->e_typ = 1.0 / (double)src->n_packets;
+        if ((rr = en->ps_minmax.ensure(2))) return rr;
+        const unsigned long long init[2] = {~0ull, 0ull}, count = (unsigned long long)(b[i + 1] - b[i]);
+        unsigned long long h[2];
+        CK(cudaMemcpyAsync(en->ps_minmax.p, init, sizeof(init), cudaMemcpyHostToDevice, en->stream));
+        const unsigned long long threads = (count + PS_CHUNK - 1) / PS_CHUNK;
+        packet_source_minmax_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, en->stream>>>(P[(size_t)i], (unsigned long long)b[i],
+                                                                                               (unsigned long long)b[i + 1], en->ps_minmax.p);
+        en->launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(h, en->ps_minmax.p, sizeof(h), cudaMemcpyDeviceToHost, en->stream));
+        CK(cudaStreamSynchronize(en->stream));
+        memcpy(&mn[(size_t)i], &h[0], sizeof(double));
+        memcpy(&mx[(size_t)i], &h[1], sizeof(double));
+        return TB200_OK;
+    });
+    if (r) return r;
+    tbps::WeightedParams W;
+    bool first = true;
+    double lo_nu = 0.0, hi_nu = 0.0;
+    for (int i = 0; i < G; i++) {
+        if (!ready[(size_t)i]) continue;
+        lo_nu = first || mn[(size_t)i] < lo_nu ? mn[(size_t)i] : lo_nu;
+        hi_nu = first || mx[(size_t)i] > hi_nu ? mx[(size_t)i] : hi_nu;
+        first = false;
+    }
+    W.nu_lo = lo_nu;
+    W.nu_range = hi_nu - lo_nu;
+    if (!std::isfinite(W.nu_range)) return fail(TB200_ERR_INVALID, "weighted source: the frequency range is not finite");
+    W.h_planck = tb::H_PLANCK;
+    W.beta_rad = 1 / (tb::K_BOLTZMANN * src->temperature);  // util/base.py:297-298
+    W.coefficient = 2 * tb::H_PLANCK / (tb::C_LIGHT * tb::C_LIGHT);
+
+    std::vector<std::vector<double>> slots((size_t)G);
+    r = each([&](int i) -> int {
+        if (!ready[(size_t)i]) return TB200_OK;
+        tb200_engine *en = m[i];
+        const uint64_t lo = (uint64_t)b[i], hi = (uint64_t)b[i + 1];
+        const size_t n_slots = (size_t)(tbps::pw_slot(hi) - tbps::pw_slot(lo) + 1);
+        int rr;
+        if ((rr = en->ps_leaf_sums.ensure(n_slots))) return rr;
+        const unsigned long long threads = (hi - lo + PS_CHUNK - 1) / PS_CHUNK;
+        packet_source_weighted_fill_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, en->stream>>>(
+            P[(size_t)i], W, lo, hi, en->in_r.p, en->in_nu.p, en->in_mu.p, en->in_energy.p, en->seeds64.p, en->ps_leaf_sums.p);
+        en->launches++;
+        CK(cudaGetLastError());
+        slots[(size_t)i].resize(n_slots);
+        CK(cudaMemcpyAsync(slots[(size_t)i].data(), en->ps_leaf_sums.p, n_slots * sizeof(double), cudaMemcpyDeviceToHost, en->stream));
+        CK(cudaStreamSynchronize(en->stream));
+        return TB200_OK;
+    });
+    if (r) return r;
+    // leaves are visited in ascending order of their start, so the member holding each one is found by walking forward
+    int owner = 0;
+    const double sum = tbps::pw_combine(0, (uint64_t)src->n_packets, [&](uint64_t s) {
+        while ((int64_t)s >= b[owner + 1]) owner++;
+        return slots[(size_t)owner][tbps::pw_slot(s) - tbps::pw_slot((uint64_t)b[owner])];
+    });
+    return each([&](int i) -> int {
+        if (!ready[(size_t)i]) return TB200_OK;
+        tb200_engine *en = m[i];
+        const long long count = b[i + 1] - b[i];
+        const long long blocks = std::min<long long>((count + 255) / 256, 4096);
+        packet_source_normalize_kernel<<<(unsigned)blocks, 256, 0, en->stream>>>(en->in_energy.p, count, sum);
+        en->launches++;
+        CK(cudaGetLastError());
+        return tb200_sync(en);
+    });
+}
+}  // extern "C++"
+
 int tb200_create_packets(tb200_engine *en, const tb200_packet_source *src) {
+    if (src && src->weighted) {
+        if (!en) return fail(TB200_ERR_INVALID, "bad argument");
+        const int64_t b[2] = {0, src->n_packets};
+        return create_weighted_packets(src, &en, b, 1, [](auto f) { return f(0); });
+    }
     return create_packets_range(en, src, 0, src ? src->n_packets : 0);
 }
 

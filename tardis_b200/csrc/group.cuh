@@ -395,6 +395,8 @@ int tb200_group_create_packets(tb200_group *g, const tb200_packet_source *src) {
     const int G = (int)g->m.size();
     std::vector<int64_t> b((size_t)G + 1);
     for (int i = 0; i <= G; i++) b[(size_t)i] = shard_lo(src->n_packets, i, G);
+    if (src->weighted)  // two sums over the whole set: the passes meet on the host (create_weighted_packets)
+        return create_weighted_packets(src, g->m.data(), b.data(), G, [&](auto f) { return group_parallel(g, &b, f); });
     return group_parallel(g, &b, [&](int i) {
         const int r = create_packets_range(g->m[(size_t)i], src, b[(size_t)i], b[(size_t)i + 1]);
         return r ? r : tb200_sync(g->m[(size_t)i]);

@@ -206,4 +206,154 @@ TB_HD int scan_chunk(const Pcg64 &origin, uint64_t k0, uint64_t k1, uint32_t rng
     return c;
 }
 
+// ---- BlackBodyWeightedSource (packet_source/black_body_weighted.py:9-108) ------------------------------------------
+// The stream after the seed segment: 5 N doubles for the Carter-Cashwell nus, which only give their min and max; N
+// doubles for rng.uniform(min, max, N) (numpy's random_uniform: lo + (hi - lo) * u); N doubles for the mus.  Energies
+// are I(nu) / sum(I) with I = intensity_black_body(nu, T) (util/base.py:279-302) and the sum in numpy's pairwise order.
+// Products and sums that numpy does not fuse are written as *_rn, so that nvcc cannot contract them into an FMA.
+TB_HD double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+TB_HD double add_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+
+struct WeightedParams {
+    double nu_lo, nu_range;  // min of the Carter-Cashwell nus, max - min (numpy forms the range once, as a double)
+    double coefficient;      // 2 h / c**2
+    double h_planck, beta_rad;  // beta_rad = 1 / (k_B T)
+};
+
+// coefficient * nu**3 / (exp(h * nu * beta_rad) - 1), evaluated left to right as numpy does.  pow and exp are the two
+// transcendentals: CUDA's and numpy's differ by about an ulp.
+TB_HD double blackbody_intensity(double nu, const WeightedParams &W) {
+    const double num = mul_rn(W.coefficient, pow(nu, 3.0));
+    const double den = add_rn(exp(mul_rn(mul_rn(W.h_planck, nu), W.beta_rad)), -1.0);
+    return num / den;
+}
+
+// min and max of the Carter-Cashwell nus of packets [i0, i1), folded into mn / mx (nothing is stored)
+TB_HD void blackbody_nu_minmax(const SourceParams &P, uint64_t i0, uint64_t i1, double &mn, double &mx) {
+    Pcg64 gx[5];
+    for (int j = 0; j < 5; j++) { gx[j] = P.origin; pcg_advance(gx[j], P.dbl_start + (uint64_t)j * P.n + i0); }
+    for (uint64_t i = i0; i < i1; i++) {
+        double xi[5];
+        for (int j = 0; j < 5; j++) xi[j] = u64_to_double(pcg_next64(gx[j]));
+        const double v = blackbody_nu(xi[0], xi[1], xi[2], xi[3], xi[4], P.l_array, P.n_l, P.l_coef, P.k_b_t, P.h_planck);
+        mn = v < mn ? v : mn;
+        mx = v > mx ? v : mx;
+    }
+}
+
+// numpy's pairwise summation of a contiguous float64 array (pairwise_sum in numpy/_core/src/umath/loops_utils.h.src):
+// a run of more than PW_BLOCK splits at n2 = n / 2 - (n / 2) % 8 and recurses; a run of 8 .. PW_BLOCK is summed by eight
+// interleaved accumulators, combined as ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7)), then its tail in order; a run
+// shorter than 8 in order.  The runs where the recursion stops -- the leaves -- depend on N alone.  Every split point is
+// a multiple of 8 and every leaf of an N > PW_BLOCK tree holds at least 64 elements, so start >> 6 names a leaf.
+constexpr uint64_t PW_BLOCK = 128;
+TB_HD uint64_t pw_split(uint64_t n) { const uint64_t n2 = n / 2; return n2 - n2 % 8; }
+TB_HD uint64_t pw_slot(uint64_t start) { return start >> 6; }
+
+// the leaf of an n-element tree that holds element p
+TB_HD void pw_leaf_at(uint64_t n, uint64_t p, uint64_t &start, uint64_t &len) {
+    uint64_t lo = 0;
+    while (n > PW_BLOCK) {
+        const uint64_t n2 = pw_split(n);
+        if (p < lo + n2) n = n2;
+        else { lo += n2; n -= n2; }
+    }
+    start = lo; len = n;
+}
+
+// The sum of an n-element tree from its leaf sums (leaf(start) -> that leaf's sum), along numpy's recursion.  Host only.
+template <class LeafSum> inline double pw_combine(uint64_t lo, uint64_t n, const LeafSum &leaf) {
+    if (n <= PW_BLOCK) return leaf(lo);
+    const uint64_t n2 = pw_split(n);
+    return pw_combine(lo, n2, leaf) + pw_combine(lo + n2, n - n2, leaf);
+}
+
+// One leaf of n elements, next() yielding them in order, summed as numpy sums it.  The eight accumulators rotate through
+// r0 .. r7 (the element's accumulator is always r0), so they stay in registers.
+template <class Next> TB_HD double pw_leaf_sum(uint64_t n, Next &next) {
+    const uint64_t m = n < 8 ? 0 : n - n % 8;
+    double r0 = 0, r1 = 0, r2 = 0, r3 = 0, r4 = 0, r5 = 0, r6 = 0, r7 = 0, res = -0.0;
+    for (uint64_t q = 0; q < n; q++) {
+        const double v = next();
+        if (q < m) {
+            const double t = q < 8 ? v : add_rn(r0, v);
+            r0 = r1; r1 = r2; r2 = r3; r3 = r4; r4 = r5; r5 = r6; r6 = r7; r7 = t;
+            if (q + 1 == m) res = add_rn(add_rn(add_rn(r0, r1), add_rn(r2, r3)), add_rn(add_rn(r4, r5), add_rn(r6, r7)));
+        } else {
+            res = add_rn(res, v);
+        }
+    }
+    return res;
+}
+
+// The weighted source's packets one after the other from packet i: seed, nu = lo + range * u, mu = sqrt(u'), radius, and
+// I(nu) in the energy slot (the caller divides by the sum).  Packet i is stored at element i - lo when lo <= i < hi.
+struct WeightedStream {
+    const SourceParams &P;
+    const WeightedParams &W;
+    uint64_t i, lo, hi;
+    double *r, *nu, *mu, *e;
+    long long *seeds;
+    Raw32 sr;
+    Pcg64 gu, gm;
+    TB_HD WeightedStream(const SourceParams &P_, const WeightedParams &W_, uint64_t i0, uint64_t lo_, uint64_t hi_, double *r_, double *nu_,
+                         double *mu_, double *e_, long long *seeds_)
+        : P(P_), W(W_), i(i0), lo(lo_), hi(hi_), r(r_), nu(nu_), mu(mu_), e(e_), seeds(seeds_) {
+        sr.seek(P.origin, raw_index_of_output(i0, P.rejected, P.n_rej));
+        gu = P.origin; pcg_advance(gu, P.dbl_start + 5ull * P.n + i0);
+        gm = P.origin; pcg_advance(gm, P.dbl_start + 6ull * P.n + i0);
+    }
+    TB_HD double operator()() {
+        uint32_t x = sr.next();
+        while (lemire_rejected(x, P.rng_excl, P.threshold)) x = sr.next();
+        const double v = add_rn(W.nu_lo, mul_rn(W.nu_range, u64_to_double(pcg_next64(gu))));
+        const double m = u64_to_double(pcg_next64(gm));
+        const double I = blackbody_intensity(v, W);
+        if (i >= lo && i < hi) {
+            const uint64_t k = i - lo;
+            if (seeds) seeds[k] = (long long)lemire_value(x, P.rng_excl);
+            if (nu) nu[k] = v;
+            if (mu) mu[k] = sqrt(m);
+            if (r) r[k] = P.radius;
+            if (e) e[k] = I;
+        }
+        i++;
+        return I;
+    }
+};
+
+// The leaves that start in [a, b), and when a == lo also the leaf holding packet lo: their packets in [lo, hi) are
+// stored (element i - lo), and every leaf that starts at or after lo leaves its sum in slots[pw_slot(start) - slot_base].
+// A leaf that runs past hi is generated to its end for its sum; those packets are not stored.
+TB_HD void weighted_fill_leaves(const SourceParams &P, const WeightedParams &W, uint64_t a, uint64_t b, uint64_t lo, uint64_t hi,
+                                double *r, double *nu, double *mu, double *e, long long *seeds, double *slots, uint64_t slot_base) {
+    uint64_t s, len;
+    pw_leaf_at(P.n, a, s, len);
+    if (s < a && a != lo) {
+        s += len;
+        if (s >= b || s >= P.n) return;
+        pw_leaf_at(P.n, s, s, len);
+    }
+    WeightedStream next(P, W, s, lo, hi, r, nu, mu, e, seeds);
+    while (true) {
+        const double sum = pw_leaf_sum(len, next);
+        if (s >= lo && slots) slots[pw_slot(s) - slot_base] = sum;
+        s += len;
+        if (s >= b || s >= P.n) break;
+        pw_leaf_at(P.n, s, s, len);
+    }
+}
+
 }  // namespace tbps

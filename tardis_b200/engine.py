@@ -342,15 +342,18 @@ class Engine:
         self._n_packets = pk.n_packets
 
     def create_packets(self, n_packets: int, seed: int, radius: float, temperature: float, l_samples: int = 1000,
-                       max_seed_val: int = 0, beta: float | None = None):
+                       max_seed_val: int = 0, beta: float | None = None, weighted: bool = False):
         """Device-side `BlackBodySimpleSource.create_packets` (packet_source/base.py:195-253, black_body.py:122-220) for
-        `np.random.default_rng(seed)`, seed = base_seed + seed_offset: the packets are generated in HBM and stay there."""
+        `np.random.default_rng(seed)`, seed = base_seed + seed_offset: the packets are generated in HBM and stay there.
+        `weighted=True`: `BlackBodyWeightedSource` (black_body_weighted.py:9-108) -- nus uniform between the extremes of a
+        plain black-body draw, energies I(nu) / sum I; needs n_packets >= 1 and no `beta`."""
         l_array = np.cumsum(np.arange(1, l_samples, dtype=np.float64) ** -4)  # black_body.py:166, numpy's own pow
         src = capi.PacketSource()
         src.n_packets = int(n_packets); src.seed = int(seed); src.radius = float(radius); src.temperature = float(temperature)
         src.l_array = l_array.ctypes.data_as(capi._pd); src.n_l = len(l_array); src.max_seed_val = int(max_seed_val)
         if beta is not None:  # BlackBodySimpleSourceRelativistic (black_body_relativistic.py:92-177)
             src.relativistic, src.beta = 1, float(beta)
+        src.weighted = int(bool(weighted))
         self._check(self._api("create_packets")(self._h, C.byref(src)))
         self._check(self._api("sync")(self._h))  # l_array may be released after this
         self._n_packets = int(n_packets)

@@ -7,6 +7,7 @@ Mirrors `BlackBodySimpleSource` (tardis/transport/montecarlo/packet_source/black
 as astropy quantities, are accepted).  The random stream is numpy's `default_rng(base_seed + seed_offset)`, reproduced on
 the device (tardis_b200/csrc/packet_source.cuh): seeds, mus, radii and energies are bit-identical to the reference's, nus
 agree to one ulp of `log`.  `legacy_mode_enabled` (the global `np.random` stream of old TARDIS versions) is not offered.
+`BlackBodyWeightedSourceB200` mirrors `BlackBodyWeightedSource` (black_body_weighted.py:9-108) the same way.
 """
 from __future__ import annotations
 
@@ -103,5 +104,40 @@ class BlackBodySimpleSourceRelativisticB200(BlackBodySimpleSourceB200):
         if not download:
             return None
         a = self.engine.download_packets()
+        return PacketCollection(a["initial_radii"], a["initial_nus"], a["initial_mus"], a["initial_energies"], a["packet_seeds"],
+                                self.calculate_radfield_luminosity())
+
+
+class BlackBodyWeightedSourceB200(BlackBodySimpleSourceB200):
+    """`BlackBodyWeightedSource` (packet_source/black_body_weighted.py:9-108) on the device: nus uniform between the min
+    and max of a plain black-body draw, each packet's energy I(nu) / sum I with I the Planck intensity, so the Wien tail
+    and the far red are sampled as densely as the peak.  Constructed by keyword only, as the reference class.  After a
+    download `self.nus` holds the frequencies, as the reference leaves them.  Seeds, radii and mus are bit-identical to
+    the reference's; nus and energies agree to the bounds INTEGRATION.md states (ulps of log, pow and exp)."""
+
+    hdf_properties = ["radius", "temperature", "base_seed"]
+    hdf_name = "black_body_weighted_source"
+
+    def __init__(self, **kwargs):
+        super().__init__(**kwargs)
+
+    def create_packets(self, no_of_packets: int, seed_offset: int = 0, *, download: bool = True):
+        """base.py:195-253 with black_body_weighted.py:55-108.  `download=False` leaves the arrays on the device only and
+        returns None."""
+        if self.radius is None or self.temperature is None:
+            raise ValueError("Black body Radius or Temperature isn't set")
+        if self.base_seed is None:
+            raise ValueError("base_seed must be set before creating packets")
+        if int(no_of_packets) == 0:  # nus.min() of the reference
+            raise ValueError("zero-size array to reduction operation minimum which has no identity")
+        if self.engine is None:
+            raise ValueError("BlackBodyWeightedSourceB200 needs the Engine that will transport the packets")
+        self.__dict__.pop("nus", None)
+        self.engine.create_packets(int(no_of_packets), int(self.base_seed) + int(seed_offset), _cgs(self.radius), _cgs(self.temperature),
+                                   max_seed_val=self.MAX_SEED_VAL, weighted=True)
+        if not download:
+            return None
+        a = self.engine.download_packets()
+        self.nus = a["initial_nus"]
         return PacketCollection(a["initial_radii"], a["initial_nus"], a["initial_mus"], a["initial_energies"], a["packet_seeds"],
                                 self.calculate_radfield_luminosity())
