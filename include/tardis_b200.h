@@ -39,6 +39,8 @@ extern "C" {
 #define TB200_ERR_MACRO_ATOM 2   /* MacroAtomError, transport/montecarlo/macro_atom.py:95 / interaction_event_callers.py:89-91 */
 #define TB200_ERR_VPACKET_LOOP 3 /* virtual packet never leaves the grid (the reference would spin in virtual_packet.py:191-243) */
 #define TB200_ERR_CONTINUUM 5    /* continuum tables inconsistent (index out of range; the reference would read out of bounds) */
+#define TB200_ERR_PLASMA_IONIZATION 6 /* PlasmaIonizationError('n_electron just turned "nan" - aborting'), plasma/properties/ion_population.py:363-366;
+                                         also the n_e fixed point not converged within its iteration cap (tb200_solve_plasma) */
 /* host-side errors */
 #define TB200_ERR_CUDA 100
 #define TB200_ERR_INVALID 101
@@ -391,7 +393,9 @@ typedef struct {
     const tb200_continuum_rows *continuum_rows;
 } tb200_atomic_data;
 typedef struct {
-    const double *level_number_density;      /* [n_levels, S] C-order (NULL with tb200_continuum_rates.beta_sobolev) */
+    const double *level_number_density;      /* [n_levels, S] C-order (NULL with tb200_continuum_rates.beta_sobolev); NULL outside
+                                                the continuum mode: the populations of the last tb200_solve_plasma since
+                                                tb200_set_model (refused when there are none) */
     double time_explosion;                   /* s (not read in the nonhomologous mode) */
     const double *j_blues;                   /* [L,S] C-order, or NULL = the table tb200_solve_radiation_field left in HBM
                                                 (only read by the macro atom's internal-up rows) */
@@ -415,6 +419,57 @@ int tb200_build_opacity(tb200_engine *engine, const tb200_plasma_state *plasma);
  * deactivation table is tb200_download_absorbing_markov's). */
 int tb200_download_opacity(tb200_engine *engine, double *tau_sobolev /* [L,S] */, double *beta_sobolev /* [L,S] */,
                            double *stimulated_emission_factor /* [L,S] */, double *transition_probabilities /* [T,S] */);
+
+/* ---- the classic plasma on the device ----
+ * Replaces the plasma update of Simulation.advance_state (simulation/base.py:363-415) for the graphs without NLTE, helium NLTE
+ * or continuum-interaction species: ionization nebular | lte, excitation dilute-lte | lte, radiative_rates_type
+ * dilute-blackbody | blackbody | detailed.  The chain (plasma/properties/general.py:20-121, partition_function.py:32-353,
+ * ion_population.py:37-390, level_population.py:13-70) and its layout: tardis_b200/csrc/plasma.cuh.
+ * Usage: tb200_set_plasma_data once, after tb200_set_atomic_data (g and metastability come from there, same level rows);
+ * then every iteration, after tb200_set_model (which uploads the host's electron densities), tb200_solve_plasma with the
+ * damped T_rad and W, and tb200_build_opacity with level_number_density == NULL.
+ * tb200_set_plasma_data refuses, before anything is allocated: levels not grouped by ion (level_ion non-decreasing, every
+ * ion with a level), ions not grouped by element in ascending atomic number with charges 0, 1, 2, ... from 0, an element
+ * with a single ion (the reference's Phi blocks would misalign), an ion of charge >= 1 without an ionisation energy, a zeta
+ * grid that is not strictly ascending or has fewer than 2 points, and the continuum mode (its plasma is the IIP one). */
+typedef struct {
+    int64_t n_levels;                 /* must equal tb200_atomic_data.n_levels */
+    const double *level_energy;       /* [n_levels] erg: levels.energy (the excitation energy) */
+    const int64_t *level_ion;         /* [n_levels] row of the level's ion in the ion table */
+    int64_t n_ions;                   /* the rows of the partition function: (atomic_number, ion_number) of the levels */
+    const int64_t *ion_atomic_number, *ion_charge; /* [n_ions] */
+    const double *ionization_energy;  /* [n_ions] erg: ionization_data of (Z, charge), the energy into this ion (charge 0: not read) */
+    int64_t n_shells;                 /* must equal the model's */
+    const double *number_density;     /* [n_elements, S] C-order, elements in the order of the ion table */
+    int64_t n_zeta_temperatures;      /* 0: no zeta table (nebular ionisation is then refused) */
+    const double *zeta_temperatures;  /* [n_zeta_temperatures] K, strictly ascending */
+    const double *zeta;               /* [n_ions, n_zeta_temperatures] C-order (rows of charge 0 not read) */
+    double chi_0;                     /* RadiationFieldCorrection's chi_0: 1.9020591570241798e-11 (Ca II), or a species' energy */
+    double k_b, h, m_e, c;            /* cgs, as tardis.constants gives them */
+} tb200_plasma_data;
+int tb200_set_plasma_data(tb200_engine *engine, const tb200_plasma_data *data);
+/* One plasma update from T_rad and W [S] (damped on the host, as in the reference).  Effects: the level populations stay in
+ * HBM for tb200_build_opacity(level_number_density == NULL); n_e becomes the model's resident electron densities (transport's
+ * chi_e, the formal integral); for dilute-blackbody / blackbody the J_blue table tb200_build_opacity(j_blues == NULL) reads
+ * is overwritten with W B_nu(T_rad) (W = 1 for blackbody); detailed keeps the table tb200_solve_radiation_field left.
+ * The n_e fixed point runs on the device in one launch and stops after 1000 iterations with TB200_ERR_PLASMA_IONIZATION
+ * (the reference's loop is unbounded); a NaN n_e gives the same code.  After an error the model's n_e and the J_blue table are
+ * unchanged and no level populations are resident.
+ * Outputs may be NULL: electron_densities [S], ion_number_density [n_ions, S], level_number_density [n_levels, S],
+ * j_blues [L, S] (the table build_opacity will read; refused if none is resident), n_e iterations (0 with fixed n_e). */
+typedef struct {
+    const double *t_radiative, *dilution_factor; /* [S] */
+    int32_t ionization;               /* 0 nebular, 1 lte */
+    int32_t excitation;               /* 0 dilute-lte, 1 lte */
+    int32_t radiative_rates_type;     /* 0 dilute-blackbody, 1 blackbody, 2 detailed */
+    double link_t_rad_t_electron;     /* T_e = link * T_rad (config plasma.link_t_rad_t_electron, 0.9) */
+    double delta_treatment;           /* NaN: delta computed; otherwise delta = this constant */
+    double departure_coefficient;     /* NaN: 1 / W */
+    double ion_zero_threshold;        /* populations below are set to 0 (1e-20) */
+    const double *electron_densities; /* [S] fixed n_e (no fixed point), or NULL */
+} tb200_plasma_params;
+int tb200_solve_plasma(tb200_engine *engine, const tb200_plasma_params *params, double *electron_densities, double *ion_number_density,
+                       double *level_number_density, double *j_blues, int32_t *iterations);
 
 /* ---- the continuum mode's macro atom on the device ----
  * Replaces steps 2-3 of ContinuumMacroAtomSolver._solve_next_macroatom_iteration (opacities/macro_atom/macroatom_solver.py:1648-1662):
@@ -491,6 +546,10 @@ int tb200_group_set_option(tb200_group *group, const char *name, int64_t value);
 int tb200_group_set_model(tb200_group *group, const tb200_model *model, const tb200_config *config);
 int tb200_group_set_atomic_data(tb200_group *group, const tb200_atomic_data *atomic);
 int tb200_group_build_opacity(tb200_group *group, const tb200_plasma_state *plasma);
+int tb200_group_set_plasma_data(tb200_group *group, const tb200_plasma_data *data);
+/* every member solves the same plasma (bit-identical results); the host outputs are member 0's */
+int tb200_group_solve_plasma(tb200_group *group, const tb200_plasma_params *params, double *electron_densities, double *ion_number_density,
+                             double *level_number_density, double *j_blues, int32_t *iterations);
 int tb200_group_build_absorbing_markov(tb200_group *group, const tb200_markov_input *input); /* every member, bit-identical tables */
 int tb200_group_upload_packets(tb200_group *group, const tb200_packets *packets);
 int tb200_group_create_packets(tb200_group *group, const tb200_packet_source *source);

@@ -21,7 +21,8 @@ EXPORTED_SYMBOLS = [
     "tb200_group_set_model", "tb200_group_set_atomic_data", "tb200_group_build_opacity", "tb200_group_upload_packets",
     "tb200_group_create_packets", "tb200_group_run", "tb200_group_run_resident", "tb200_group_sync", "tb200_group_allreduce",
     "tb200_group_allreduce_ms", "tb200_group_formal_integral", "tb200_group_formal_integral_ms",
-    "tb200_group_build_absorbing_markov",
+    "tb200_group_build_absorbing_markov", "tb200_set_plasma_data", "tb200_solve_plasma", "tb200_group_set_plasma_data",
+    "tb200_group_solve_plasma",
 ]
 
 
@@ -143,6 +144,25 @@ class PlasmaState(C.Structure):
                 ("continuum", C.POINTER(ContinuumRates))]
 
 
+class PlasmaData(C.Structure):
+    """tb200_plasma_data"""
+    _fields_ = [
+        ("n_levels", C.c_int64), ("level_energy", _pd), ("level_ion", _pi), ("n_ions", C.c_int64), ("ion_atomic_number", _pi),
+        ("ion_charge", _pi), ("ionization_energy", _pd), ("n_shells", C.c_int64), ("number_density", _pd),
+        ("n_zeta_temperatures", C.c_int64), ("zeta_temperatures", _pd), ("zeta", _pd), ("chi_0", C.c_double),
+        ("k_b", C.c_double), ("h", C.c_double), ("m_e", C.c_double), ("c", C.c_double),
+    ]
+
+
+class PlasmaParams(C.Structure):
+    """tb200_plasma_params"""
+    _fields_ = [
+        ("t_radiative", _pd), ("dilution_factor", _pd), ("ionization", C.c_int32), ("excitation", C.c_int32),
+        ("radiative_rates_type", C.c_int32), ("link_t_rad_t_electron", C.c_double), ("delta_treatment", C.c_double),
+        ("departure_coefficient", C.c_double), ("ion_zero_threshold", C.c_double), ("electron_densities", _pd),
+    ]
+
+
 class MarkovInput(C.Structure):
     """tb200_markov_input"""
     _fields_ = [
@@ -242,6 +262,10 @@ def load(build_if_missing: bool = True):
     lib.tb200_build_absorbing_markov.argtypes = [E, C.POINTER(MarkovInput)]
     lib.tb200_download_absorbing_markov.argtypes = [E, _pd, _pd]
     lib.tb200_group_build_absorbing_markov.argtypes = [E, C.POINTER(MarkovInput)]
+    lib.tb200_set_plasma_data.argtypes = [E, C.POINTER(PlasmaData)]
+    lib.tb200_solve_plasma.argtypes = [E, C.POINTER(PlasmaParams), _pd, _pd, _pd, _pd, C.POINTER(C.c_int32)]
+    lib.tb200_group_set_plasma_data.argtypes = [E, C.POINTER(PlasmaData)]
+    lib.tb200_group_solve_plasma.argtypes = [E, C.POINTER(PlasmaParams), _pd, _pd, _pd, _pd, C.POINTER(C.c_int32)]
     lib.tb200_group_create.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(E)]
     lib.tb200_group_destroy.argtypes = [E]
     lib.tb200_group_destroy.restype = None
@@ -266,7 +290,7 @@ def load(build_if_missing: bool = True):
                  "tb200_set_atomic_data", "tb200_build_opacity", "tb200_download_opacity", "tb200_line_accumulators",
                  "tb200_finalize_line_estimators", "tb200_run_resident",
                  "tb200_solve_source_function", "tb200_formal_integral", "tb200_formal_integral_ms",
-                 "tb200_build_absorbing_markov", "tb200_download_absorbing_markov",
+                 "tb200_build_absorbing_markov", "tb200_download_absorbing_markov", "tb200_set_plasma_data", "tb200_solve_plasma",
                  *(n for n in EXPORTED_SYMBOLS if n.startswith("tb200_group_") and n != "tb200_group_destroy")):
         getattr(lib, name).restype = C.c_int
     _lib = lib

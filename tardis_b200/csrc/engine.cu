@@ -21,6 +21,7 @@
 #include "formal_integral.cuh"
 #include "markov_build.cuh"
 #include "nonhomologous.cuh"
+#include "plasma.cuh"
 
 namespace {
 
@@ -150,6 +151,19 @@ struct tb200_engine {
     DBuf<unsigned char> at_meta, at_nlte;
     DBuf<double> at_g, at_wfl, at_flu, at_ful, at_elo, at_eup, op_lnd, op_beta_t, op_stim_t, op_tp_norm_t;
     DBuf<double> op_dvdr;  // [S] the caller's velocity_gradient of tb200_build_opacity (nonhomologous mode)
+    // classic plasma (plasma.cuh): the tables of tb200_set_plasma_data, per-iteration work arrays.  The level populations
+    // of tb200_solve_plasma lie in op_lnd, where tb200_build_opacity reads them.
+    bool pl_set = false;            // tb200_set_plasma_data has been given (for pl_S shells and pl_n_levels levels)
+    bool pl_valid = false;          // op_lnd holds the populations of a tb200_solve_plasma since the last tb200_set_model
+    int pl_S = 0, pl_n_ions = 0, pl_n_elements = 0;
+    int64_t pl_n_levels = 0;
+    double pl_chi_0 = 0.0;
+    tbp::Constants pl_const{};
+    double pl_c = 0.0;
+    std::vector<double> pl_zeta_t;  // zeta temperature grid (the interpolation weights are set up on the host)
+    DBuf<double> pl_energy, pl_charge, pl_chi, pl_nd, pl_zeta, pl_z, pl_phi, pl_pop, pl_ne, pl_new, pl_fixed_ne;
+    DBuf<int> pl_level_ion, pl_ion_first, pl_element_first, pl_status;
+    DBuf<tbp::Shell> pl_shell;
     // control
     DBuf<unsigned> rng_buf;
     DBuf<unsigned long long> ctrl;  // [0] next_packet, [1] vlog_count, [2..] counters
@@ -320,6 +334,7 @@ int tb200_set_model(tb200_engine *en, const tb200_model *m, const tb200_config *
     }
     en->have_model = false;
     en->sf_valid = false;
+    en->pl_valid = false;
     en->diff_scale1 = en->diff_scale2 = 0.0;  // the difference arrays are zeroed below
     en->S = (int)m->n_shells; en->L = (int)m->n_lines; en->lpad = round_up(en->L, 32) + 32;
     en->T = (int)m->n_transitions; en->tpad = round_up(en->T > 0 ? en->T : 1, 32); en->n_blocks = (int)m->n_blocks;
@@ -2005,9 +2020,13 @@ static int wait_opacity_build(tb200_engine *en) {
 int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
     // continuum rates with beta / stim: the line rows read the caller's tables, tau is the model's (not rebuilt)
     const bool host_lines = p && p->continuum && (p->continuum->beta_sobolev || p->continuum->stimulated_emission_factor);
-    if (!en || !p || (!p->level_number_density && !host_lines)) return fail(TB200_ERR_INVALID, "bad argument");
+    if (!en || !p) return fail(TB200_ERR_INVALID, "bad argument");
     if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
     if (!en->have_atomic) return fail(TB200_ERR_NO_MODEL, "tb200_set_atomic_data has not been called");
+    // level_number_density NULL: the populations tb200_solve_plasma left in op_lnd
+    const bool resident_lnd = !p->level_number_density && !host_lines;
+    if (resident_lnd && !en->pl_valid)
+        return fail(TB200_ERR_INVALID, "level_number_density is NULL and no tb200_solve_plasma since tb200_set_model has left populations in HBM");
     if (!en->continuum && p->continuum) return fail(TB200_ERR_INVALID, "continuum: the continuum mode's rates; this model has no continuum");
     if (en->continuum) {
         const tb200_continuum_rates *cr = p->continuum;
@@ -2047,7 +2066,10 @@ int tb200_build_opacity(tb200_engine *en, const tb200_plasma_state *p) {
             return r;
     } else {
         if ((r = en->op_lnd.ensure((size_t)en->n_levels * S)) || (r = en->op_beta_t.ensure((size_t)S * lpad)) || (r = en->op_stim_t.ensure((size_t)S * lpad))) return r;
-        CK(cudaMemcpyAsync(en->op_lnd.p, p->level_number_density, (size_t)en->n_levels * S * sizeof(double), cudaMemcpyHostToDevice, st));
+        if (!resident_lnd) {
+            en->pl_valid = false;  // op_lnd now holds the caller's populations
+            CK(cudaMemcpyAsync(en->op_lnd.p, p->level_number_density, (size_t)en->n_levels * S * sizeof(double), cudaMemcpyHostToDevice, st));
+        }
         const long long total = (long long)S * lpad;
         const unsigned grid = (unsigned)((total + 255) / 256);
         if (en->nonhomologous) {
@@ -2132,6 +2154,246 @@ int tb200_download_opacity(tb200_engine *en, double *tau, double *beta, double *
         if ((r = download_line_major(en, kept, en->T, en->tpad, tp))) return r;
         CK(cudaStreamSynchronize(st));
     }
+    return TB200_OK;
+}
+
+// ---- classic plasma on the device (plasma.cuh) --------------------------------------------------------------------------
+namespace {
+// (level, shell): the Boltzmann factors, into op_lnd (overwritten in place by the populations at the end)
+__global__ void plasma_boltzmann_kernel(const tbp::Shell *sh, const double *g, const unsigned char *meta, const double *energy,
+                                        long long n_levels, int n_shells, int dilute, double *lbf) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_levels * n_shells) return;
+    const long long l = i / n_shells;
+    const int s = (int)(i % n_shells);
+    lbf[i] = tbp::boltzmann_factor(g[l], energy[l], sh[s].beta_rad, sh[s].w, dilute && !meta[l]);
+}
+// (ion, shell): the partition function, then Phi of every ion of charge >= 1 (0 in the rows of charge 0, never read)
+__global__ void plasma_partition_kernel(const double *lbf, const int *ion_first, int n_ions, int n_shells, double *z) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n_ions * n_shells) return;
+    const int ion = (int)(i / n_shells), s = (int)(i % n_shells);
+    z[i] = tbp::partition_function(lbf, ion_first[ion], ion_first[ion + 1], n_shells, s);
+}
+__global__ void plasma_phi_kernel(const tbp::Shell *sh, const double *z, const double *charge, const double *chi, const double *zeta, int n_t,
+                                  int n_ions, int n_shells, int nebular, double chi_0, double delta_treatment, double *phi) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n_ions * n_shells) return;
+    const int ion = (int)(i / n_shells), s = (int)(i % n_shells);
+    if (charge[ion] == 0.0) { phi[i] = 0.0; return; }
+    const tbp::Shell h = sh[s];
+    double p = tbp::phi_lte(z[i], z[i - n_shells], h.g_e, chi[ion], h.beta_rad);
+    if (nebular)
+        p = tbp::phi_nebular(h, p, tbp::zeta_value(h, zeta + (size_t)ion * n_t), tbp::radiation_field_correction(h, chi[ion], chi_0, delta_treatment));
+    phi[i] = p;
+}
+// The n_e fixed point in one CTA (tbp::ne_fixed_point): the threads share out the (element, shell) population blocks and
+// the shells; the all-shells test is a block-wide AND.  status = {population passes, tbp::NeStatus}.
+constexpr int NE_THREADS = 1024;
+extern "C++" {  // a template, inside the C-ABI block
+struct CtaTeam {
+    template <class F> __device__ void each(int n, F f) { for (int i = threadIdx.x; i < n; i += blockDim.x) f(i); }
+    __device__ void sync() { __syncthreads(); }
+    __device__ bool any(bool v) { return __syncthreads_or(v) != 0; }
+    __device__ bool all(bool v) { return __syncthreads_and(v) != 0; }
+};
+}  // extern "C++"
+__global__ void __launch_bounds__(NE_THREADS) plasma_ne_kernel(const double *phi, const double *nd, const int *element_first, int n_elements,
+                                                               const double *charge, int n_ions, int n_shells, double threshold,
+                                                               const double *fixed_ne, double *pop, double *ne, double *new_ne, int *status) {
+    CtaTeam team;
+    int passes = 0;
+    const tbp::NeStatus r = tbp::ne_fixed_point(team, phi, nd, element_first, n_elements, charge, n_ions, n_shells, threshold, fixed_ne, pop, ne,
+                                                new_ne, &passes);
+    if (threadIdx.x == 0) { status[0] = passes; status[1] = (int)r; }
+}
+// (level, shell): Boltzmann factor -> population, in place
+__global__ void plasma_level_kernel(const int *level_ion, const double *z, const double *pop, long long n_levels, int n_shells, double *lnd) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_levels * n_shells) return;
+    const long long l = i / n_shells;
+    const size_t c = (size_t)level_ion[l] * n_shells + (size_t)(i % n_shells);
+    lnd[i] = tbp::level_population(lnd[i], z[c], pop[c]);
+}
+// (shell, line) of the [S][lpad] table the opacity build reads: W B_nu(T_rad) (W = 1 for the black body), 0 in the padding
+__global__ void plasma_jblue_kernel(tbr::Constants K, const tbp::Shell *sh, const double *nu_line, int n_lines, int lpad, int n_shells, int blackbody,
+                                    double *out_t) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n_shells * lpad) return;
+    const int s = (int)(i / lpad), l = (int)(i % lpad);
+    out_t[i] = l < n_lines ? tbr::dilute_planck_intensity(K, nu_line[l], sh[s].t_rad, blackbody ? 1.0 : sh[s].w) : 0.0;
+}
+inline unsigned blocks_for(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+}  // namespace
+
+int tb200_set_plasma_data(tb200_engine *en, const tb200_plasma_data *d) {
+    if (!en || !d) return fail(TB200_ERR_INVALID, "bad argument");
+    if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
+    if (en->continuum) return fail(TB200_ERR_INVALID, "plasma data: the continuum mode's plasma is the IIP one, which tb200_solve_plasma does not build");
+    if (!en->have_atomic) return fail(TB200_ERR_NO_MODEL, "tb200_set_atomic_data has not been called (g and metastability come from it)");
+    if (d->n_levels != en->n_levels) return fail(TB200_ERR_INVALID, "plasma data: n_levels differs from the atomic data's");
+    if (d->n_shells != en->S) return fail(TB200_ERR_INVALID, "plasma data: n_shells differs from the model's");
+    if (!d->level_energy || !d->level_ion || !d->ion_atomic_number || !d->ion_charge || !d->ionization_energy || !d->number_density)
+        return fail(TB200_ERR_INVALID, "plasma data: missing array");
+    if (d->n_ions < 2 || d->n_ions > d->n_levels) return fail(TB200_ERR_INVALID, "plasma data: n_ions out of range");
+    const int64_t NL = d->n_levels, NI = d->n_ions;
+    // levels grouped by ion, in the ion table's order, every ion with at least one level (the partition function's rows)
+    std::vector<int> ion_first((size_t)NI + 1, 0);
+    for (int64_t l = 0; l < NL; l++) {
+        const int64_t ion = d->level_ion[l], prev = l ? d->level_ion[l - 1] : -1;
+        if (ion < 0 || ion >= NI) return fail(TB200_ERR_INVALID, "plasma data: level_ion of level " + std::to_string(l) + " is out of range");
+        if (ion != prev && ion != prev + 1)
+            return fail(TB200_ERR_INVALID, "plasma data: levels are not grouped by (atomic_number, ion_number) in the ion table's order (level " +
+                                               std::to_string(l) + ")");
+        if (ion != prev) ion_first[(size_t)ion] = (int)l;
+    }
+    if (d->level_ion[NL - 1] != NI - 1) return fail(TB200_ERR_INVALID, "plasma data: an ion of the ion table has no level");
+    ion_first[(size_t)NI] = (int)NL;
+    // ions grouped by element in ascending atomic number, charges 0, 1, 2, ... in each; at least two ions per element
+    std::vector<int> element_first;
+    std::vector<double> charge((size_t)NI);
+    for (int64_t i = 0; i < NI; i++) {
+        const bool first = i == 0 || d->ion_atomic_number[i] != d->ion_atomic_number[i - 1];
+        if (first) {
+            if (i > 0 && d->ion_atomic_number[i] < d->ion_atomic_number[i - 1])
+                return fail(TB200_ERR_INVALID, "plasma data: ions are not grouped by element in ascending atomic number (ion " + std::to_string(i) + ")");
+            if (d->ion_charge[i] != 0)
+                return fail(TB200_ERR_INVALID, "plasma data: the ions of atomic number " + std::to_string(d->ion_atomic_number[i]) +
+                                                   " do not start from charge 0");
+            if (i > 0 && i - element_first.back() < 2)
+                return fail(TB200_ERR_INVALID, "plasma data: atomic number " + std::to_string(d->ion_atomic_number[i - 1]) +
+                                                   " has a single ion (its Phi block would be empty and the elements' rows misalign)");
+            element_first.push_back((int)i);
+        } else {
+            if (d->ion_charge[i] != d->ion_charge[i - 1] + 1)
+                return fail(TB200_ERR_INVALID, "plasma data: the ions of atomic number " + std::to_string(d->ion_atomic_number[i]) +
+                                                   " are not consecutive in charge (ion " + std::to_string(i) + ")");
+            if (d->ionization_energy[i] != d->ionization_energy[i])
+                return fail(TB200_ERR_INVALID, "plasma data: ion (" + std::to_string(d->ion_atomic_number[i]) + ", " + std::to_string(d->ion_charge[i]) +
+                                                   ") has no ionisation energy (a Phi row without one)");
+        }
+        charge[(size_t)i] = (double)d->ion_charge[i];
+    }
+    if (NI - element_first.back() < 2)
+        return fail(TB200_ERR_INVALID, "plasma data: atomic number " + std::to_string(d->ion_atomic_number[NI - 1]) + " has a single ion");
+    const int n_elements = (int)element_first.size();
+    element_first.push_back((int)NI);
+    const int64_t NT = d->n_zeta_temperatures;
+    if (NT < 0 || NT == 1) return fail(TB200_ERR_INVALID, "plasma data: the zeta grid needs at least 2 temperatures (or 0: none)");
+    if (NT > 0) {
+        if (!d->zeta_temperatures || !d->zeta) return fail(TB200_ERR_INVALID, "plasma data: zeta_temperatures or zeta is NULL");
+        for (int64_t k = 1; k < NT; k++)
+            if (!(d->zeta_temperatures[k] > d->zeta_temperatures[k - 1]))
+                return fail(TB200_ERR_INVALID, "plasma data: zeta_temperatures must be strictly ascending");
+    }
+    CK(cudaSetDevice(en->device));
+    en->pl_set = false;
+    const int S = en->S;
+    cudaStream_t st = en->stream;
+    int r;
+    if ((r = en->pl_energy.ensure(NL)) || (r = en->pl_level_ion.ensure(NL)) || (r = en->pl_ion_first.ensure(NI + 1)) || (r = en->pl_charge.ensure(NI)) ||
+        (r = en->pl_chi.ensure(NI)) || (r = en->pl_element_first.ensure(element_first.size())) || (r = en->pl_nd.ensure((size_t)n_elements * S)) ||
+        (r = en->pl_zeta.ensure((size_t)std::max<int64_t>(NT, 1) * NI)) || (r = en->pl_z.ensure((size_t)NI * S)) || (r = en->pl_phi.ensure((size_t)NI * S)) ||
+        (r = en->pl_pop.ensure((size_t)NI * S)) || (r = en->pl_ne.ensure(S)) || (r = en->pl_new.ensure(S)) || (r = en->pl_fixed_ne.ensure(S)) ||
+        (r = en->pl_status.ensure(2)) || (r = en->pl_shell.ensure(S)))
+        return r;
+    std::vector<int> level_ion((size_t)NL);
+    for (int64_t l = 0; l < NL; l++) level_ion[(size_t)l] = (int)d->level_ion[l];
+    CK(cudaMemcpyAsync(en->pl_energy.p, d->level_energy, NL * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(en->pl_level_ion.p, level_ion.data(), NL * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(en->pl_ion_first.p, ion_first.data(), (NI + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(en->pl_charge.p, charge.data(), NI * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(en->pl_chi.p, d->ionization_energy, NI * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(en->pl_element_first.p, element_first.data(), element_first.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(en->pl_nd.p, d->number_density, (size_t)n_elements * S * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (NT > 0) CK(cudaMemcpyAsync(en->pl_zeta.p, d->zeta, (size_t)NT * NI * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));  // the host vectors go out of scope
+    en->pl_zeta_t.assign(d->zeta_temperatures, d->zeta_temperatures + NT);
+    en->pl_S = S; en->pl_n_levels = NL; en->pl_n_ions = (int)NI; en->pl_n_elements = n_elements;
+    en->pl_chi_0 = d->chi_0;
+    en->pl_const = tbp::Constants{d->k_b, d->h, d->m_e};
+    en->pl_c = d->c;
+    en->pl_valid = false;
+    en->pl_set = true;
+    return TB200_OK;
+}
+
+int tb200_solve_plasma(tb200_engine *en, const tb200_plasma_params *p, double *electron_densities, double *ion_number_density,
+                       double *level_number_density, double *j_blues, int32_t *iterations) {
+    if (!en || !p || !p->t_radiative || !p->dilution_factor) return fail(TB200_ERR_INVALID, "bad argument");
+    if (!en->have_model) return fail(TB200_ERR_NO_MODEL, "tb200_set_model has not been called");
+    if (en->continuum) return fail(TB200_ERR_INVALID, "the continuum mode's plasma is the IIP one, which tb200_solve_plasma does not build");
+    if (!en->pl_set) return fail(TB200_ERR_NO_MODEL, "tb200_set_plasma_data has not been called");
+    if (en->pl_S != en->S || en->pl_n_levels != en->n_levels)
+        return fail(TB200_ERR_NO_MODEL, "the plasma data were given for another shell or level count: call tb200_set_plasma_data again");
+    if (p->ionization < 0 || p->ionization > 1 || p->excitation < 0 || p->excitation > 1 || p->radiative_rates_type < 0 || p->radiative_rates_type > 2)
+        return fail(TB200_ERR_INVALID, "ionization must be 0 (nebular) or 1 (lte), excitation 0 (dilute-lte) or 1 (lte), radiative_rates_type 0, 1 or 2");
+    const bool nebular = p->ionization == 0, detailed = p->radiative_rates_type == 2;
+    if (nebular && en->pl_zeta_t.empty()) return fail(TB200_ERR_INVALID, "nebular ionisation needs the zeta table of tb200_set_plasma_data");
+    if (detailed && j_blues && !en->rf_valid) return fail(TB200_ERR_INVALID, "j_blues: detailed keeps tb200_solve_radiation_field's table, and none is resident");
+    const int S = en->S, L = en->L, lpad = en->lpad, NI = en->pl_n_ions;
+    const long long NL = en->n_levels;
+    // DilutePlanckianRadiationField's checks (plasma/radiation_field/planck_rad_field.py:46-48)
+    for (int s = 0; s < S; s++)
+        if (!(p->t_radiative[s] > 0 && std::isfinite(p->t_radiative[s])) || !(p->dilution_factor[s] >= 0 && std::isfinite(p->dilution_factor[s])))
+            return fail(TB200_ERR_INVALID, "t_radiative must be positive and dilution_factor non-negative, both finite (shell " + std::to_string(s) + ")");
+    std::vector<tbp::Shell> shells((size_t)S);
+    const std::vector<double> &grid = en->pl_zeta_t;
+    const int NT = (int)grid.size();
+    for (int s = 0; s < S; s++) {
+        tbp::Shell &h = shells[(size_t)s];
+        h = tbp::shell_state(en->pl_const, p->t_radiative[s], p->dilution_factor[s], p->link_t_rad_t_electron, p->departure_coefficient);
+        if (NT >= 2) {  // interp1d(bounds_error=False, fill_value=nan): NaN outside [grid[0], grid[-1]]
+            const tbfi::ShellWeights w = tbfi::shell_weights(grid.data(), NT, h.t_rad);
+            h.z_lo = w.lo; h.z_w_lo = w.w_lo; h.z_w_hi = w.w_hi;
+            h.z_out = h.t_rad < grid[0] || h.t_rad > grid[(size_t)NT - 1];
+        }
+    }
+    CK(cudaSetDevice(en->device));
+    int r;
+    if ((r = en->op_lnd.ensure((size_t)NL * S))) return r;
+    if (!detailed && (r = en->rf_jblues_t.ensure((size_t)S * lpad))) return r;
+    cudaStream_t st = en->stream;
+    en->pl_valid = false;  // op_lnd is rebuilt from here on
+    CK(cudaMemcpyAsync(en->pl_shell.p, shells.data(), (size_t)S * sizeof(tbp::Shell), cudaMemcpyHostToDevice, st));
+    if (p->electron_densities) CK(cudaMemcpyAsync(en->pl_fixed_ne.p, p->electron_densities, (size_t)S * sizeof(double), cudaMemcpyHostToDevice, st));
+    const long long level_cells = NL * S, ion_cells = (long long)NI * S;
+    plasma_boltzmann_kernel<<<blocks_for(level_cells, 256), 256, 0, st>>>(en->pl_shell.p, en->at_g.p, en->at_meta.p, en->pl_energy.p, NL, S,
+                                                                          p->excitation == 0, en->op_lnd.p);
+    plasma_partition_kernel<<<blocks_for(ion_cells, 128), 128, 0, st>>>(en->op_lnd.p, en->pl_ion_first.p, NI, S, en->pl_z.p);
+    plasma_phi_kernel<<<blocks_for(ion_cells, 128), 128, 0, st>>>(en->pl_shell.p, en->pl_z.p, en->pl_charge.p, en->pl_chi.p, en->pl_zeta.p, NT, NI, S,
+                                                                  nebular, en->pl_chi_0, p->delta_treatment, en->pl_phi.p);
+    plasma_ne_kernel<<<1, NE_THREADS, 0, st>>>(en->pl_phi.p, en->pl_nd.p, en->pl_element_first.p, en->pl_n_elements, en->pl_charge.p, NI, S,
+                                               p->ion_zero_threshold, p->electron_densities ? en->pl_fixed_ne.p : nullptr, en->pl_pop.p, en->pl_ne.p,
+                                               en->pl_new.p, en->pl_status.p);
+    en->launches += 4;
+    CK(cudaGetLastError());
+    int status[2] = {0, 0};
+    CK(cudaMemcpyAsync(status, en->pl_status.p, sizeof(status), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (iterations) *iterations = status[0];
+    if (status[1] == tbp::NE_NAN) return fail(TB200_ERR_PLASMA_IONIZATION, "n_electron just turned \"nan\" - aborting");
+    if (status[1] == tbp::NE_CAP)
+        return fail(TB200_ERR_PLASMA_IONIZATION, "n_electron did not converge within " + std::to_string(tbp::MAX_NE_ITERATIONS) +
+                                                     " iterations - aborting (the device's cap; the reference has none)");
+    plasma_level_kernel<<<blocks_for(level_cells, 256), 256, 0, st>>>(en->pl_level_ion.p, en->pl_z.p, en->pl_pop.p, NL, S, en->op_lnd.p);
+    en->launches++;
+    if (!detailed) {
+        tbr::Constants K{};
+        K.c = en->pl_c; K.h = en->pl_const.h; K.k_b = en->pl_const.k_b;
+        plasma_jblue_kernel<<<blocks_for((long long)S * lpad, 256), 256, 0, st>>>(K, en->pl_shell.p, en->nu_line.p, L, lpad, S,
+                                                                                  p->radiative_rates_type == 1, en->rf_jblues_t.p);
+        en->launches++;
+    }
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(en->n_e.p, en->pl_ne.p, (size_t)S * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (electron_densities) CK(cudaMemcpyAsync(electron_densities, en->pl_ne.p, (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (ion_number_density) CK(cudaMemcpyAsync(ion_number_density, en->pl_pop.p, (size_t)ion_cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (level_number_density) CK(cudaMemcpyAsync(level_number_density, en->op_lnd.p, (size_t)level_cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (j_blues && (r = download_line_major(en, en->rf_jblues_t.p, L, lpad, j_blues))) return r;
+    CK(cudaStreamSynchronize(st));
+    en->pl_valid = true;
+    if (!detailed) en->rf_valid = true;
     return TB200_OK;
 }
 

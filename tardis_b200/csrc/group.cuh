@@ -363,6 +363,20 @@ int tb200_group_build_opacity(tb200_group *g, const tb200_plasma_state *plasma) 
     });
 }
 
+int tb200_group_set_plasma_data(tb200_group *g, const tb200_plasma_data *data) {
+    if (!g) return fail(TB200_ERR_INVALID, "bad argument");
+    return group_parallel(g, nullptr, [&](int i) { return tb200_set_plasma_data(g->m[(size_t)i], data); });
+}
+
+int tb200_group_solve_plasma(tb200_group *g, const tb200_plasma_params *params, double *electron_densities, double *ion_number_density,
+                             double *level_number_density, double *j_blues, int32_t *iterations) {
+    if (!g) return fail(TB200_ERR_INVALID, "bad argument");
+    return group_parallel(g, nullptr, [&](int i) {
+        if (i == 0) return tb200_solve_plasma(g->m[0], params, electron_densities, ion_number_density, level_number_density, j_blues, iterations);
+        return tb200_solve_plasma(g->m[(size_t)i], params, nullptr, nullptr, nullptr, nullptr, nullptr);
+    });
+}
+
 int tb200_group_build_absorbing_markov(tb200_group *g, const tb200_markov_input *input) {
     if (!g) return fail(TB200_ERR_INVALID, "bad argument");
     return group_parallel(g, nullptr, [&](int i) { return tb200_build_absorbing_markov(g->m[(size_t)i], input); });

@@ -28,8 +28,21 @@ class MacroAtomError(ValueError):
     """Same name and base as tardis/transport/montecarlo/macro_atom.py:15."""
 
 
+class PlasmaException(Exception):
+    """Same name and base as tardis/plasma/exceptions.py:1."""
+
+
+class PlasmaIonizationError(PlasmaException):
+    """Same name and base as tardis/plasma/exceptions.py:25 (n_e turned NaN, or did not converge within the device's cap)."""
+
+
 class EngineError(RuntimeError):
     pass
+
+
+IONIZATION = {"nebular": 0, "lte": 1}
+EXCITATION = {"dilute-lte": 0, "lte": 1}
+RADIATIVE_RATES_TYPE = {"dilute-blackbody": 0, "blackbody": 1, "detailed": 2}
 
 
 _pd = C.POINTER(C.c_double)
@@ -65,6 +78,7 @@ class Engine:
         self._n_packets = 0
         self._n_continua = 0
         self._n_markov = 0
+        self._plasma_shape = None
         self._keep = []
 
     # ---- plumbing ----
@@ -82,6 +96,8 @@ class Engine:
             raise MacroAtomError(msg)
         if code == 5:
             raise MonteCarloException(msg)
+        if code == 6:
+            raise PlasmaIonizationError(msg)
         raise EngineError(f"tb200 error {code}: {msg}")
 
     def close(self):
@@ -419,7 +435,8 @@ class Engine:
 
     def build_opacity(self, level_number_density, time_explosion, j_blues=None, velocity_gradient=None, continuum=None):
         """`tb200_build_opacity`: tau_Sobolev, beta_Sobolev and the normalised macro-atom probabilities of this iteration, built
-        in HBM from the level populations [n_levels, S] (and J_blue: `None` = the table `solve_radiation_field` left resident).
+        in HBM from the level populations [n_levels, S] (`None` outside the continuum mode: the populations `solve_plasma` left
+        resident) and J_blue (`None` = the table `solve_radiation_field` or `solve_plasma` left resident).
         `velocity_gradient` [S] (1/s): the nonhomologous mode's tau (modes/nonhomologous/tau_sobolev.py:21-75), required for a
         nonhomologous model, whose `time_explosion` is then not read.  `continuum` (continuum mode only, required there): the
         macro atom's rates of this iteration, a dict of rate (6 arrays [key, S]), cooling (3 arrays [key, S]: the reference's
@@ -469,6 +486,82 @@ class Engine:
                     setattr(cr, k, _dptr(t))
             p.continuum = C.pointer(cr)
         self._check(self._api("build_opacity")(self._h, C.byref(p)))
+
+    # ---- the classic plasma on the device ----
+    def set_plasma_data(self, *, level_energy, level_ion, ion_atomic_number, ion_charge, ionization_energy, number_density,
+                        zeta_temperatures=None, zeta=None, chi_0=1.9020591570241798e-11):
+        """`tb200_set_plasma_data`, once after `set_atomic_data` (whose g and metastability it uses, same level rows): per level
+        its excitation energy and ion row, the ion table (atomic number, charge, ionisation energy into the ion; NaN for
+        charge 0), number_density [n_elements, S] in the ion table's element order, the zeta table [n_ions, n_T] on its
+        temperature grid (nebular ionisation only) and chi_0.  `tardis_b200.plasma.plasma_data` derives all of it from the
+        reference's frames."""
+        lev_e, lev_ion = _f64(level_energy), _i64(level_ion)
+        z, q, chi = _i64(ion_atomic_number), _i64(ion_charge), _f64(ionization_energy)
+        nd = _f64(number_density)
+        if len(lev_e) != len(lev_ion) or not len(z) == len(q) == len(chi) or nd.ndim != 2:
+            raise ValueError("plasma data: one energy and ion row per level, one atomic number / charge / energy per ion, "
+                             "number_density [n_elements, n_shells]")
+        d = capi.PlasmaData()
+        d.n_levels, d.level_energy, d.level_ion = len(lev_e), _dptr(lev_e), _iptr(lev_ion)
+        d.n_ions, d.ion_atomic_number, d.ion_charge, d.ionization_energy = len(z), _iptr(z), _iptr(q), _dptr(chi)
+        d.n_shells, d.number_density = nd.shape[1], _dptr(nd)
+        keep = [lev_e, lev_ion, z, q, chi, nd]
+        if zeta is not None:
+            zt, zz = _f64(zeta_temperatures), _f64(zeta)
+            if zz.shape != (len(z), len(zt)):
+                raise ValueError(f"zeta must be [n_ions, n_temperatures] = [{len(z)}, {len(zt)}], got {zz.shape}")
+            d.n_zeta_temperatures, d.zeta_temperatures, d.zeta = len(zt), _dptr(zt), _dptr(zz)
+            keep += [zt, zz]
+        d.chi_0 = float(chi_0)
+        d.k_b, d.h, d.m_e, d.c = 1.3806488e-16, 6.62606957e-27, 9.10938291e-28, 2.99792458e10  # CODATA-2010 cgs (tardis/constants.py:1)
+        self._check(self._api("set_plasma_data")(self._h, C.byref(d)))
+        self._plasma_shape = (len(lev_e), len(z))
+
+    def solve_plasma(self, t_radiative, dilution_factor, *, ionization="nebular", excitation="dilute-lte",
+                     radiative_rates_type="dilute-blackbody", link_t_rad_t_electron=0.9, delta_treatment=None,
+                     departure_coefficient=None, ion_zero_threshold=1e-20, electron_densities=None, download=False):
+        """`tb200_solve_plasma`: level populations, ion populations, n_e and (dilute-blackbody / blackbody) the J_blue table from
+        the damped T_rad and W [S].  The populations stay in HBM for `build_opacity(None, ...)`, n_e becomes the model's
+        electron densities, J_blue the table `build_opacity(..., j_blues=None)` reads.  `electron_densities` [S]: fixed n_e
+        (no fixed point).  A NaN n_e, or no convergence within 1000 iterations, raises PlasmaIonizationError.
+        download=True returns a dict of electron_densities [S], ion_number_density [n_ions, S], level_number_density
+        [n_levels, S], j_blues [L, S] and iterations; otherwise only iterations."""
+        L, S, _ = self._model_shape
+        t, w = _f64(t_radiative), _f64(dilution_factor)
+        if t.shape != (S,) or w.shape != (S,):
+            raise ValueError(f"t_radiative and dilution_factor need one entry per shell ({S})")
+        for name, table, v in (("ionization", IONIZATION, ionization), ("excitation", EXCITATION, excitation),
+                               ("radiative_rates_type", RADIATIVE_RATES_TYPE, radiative_rates_type)):
+            if v not in table:
+                raise ValueError(f"{name} must be one of {sorted(table)}, got {v!r}")
+        p = capi.PlasmaParams()
+        p.t_radiative, p.dilution_factor = _dptr(t), _dptr(w)
+        p.ionization, p.excitation = IONIZATION[ionization], EXCITATION[excitation]
+        p.radiative_rates_type = RADIATIVE_RATES_TYPE[radiative_rates_type]
+        p.link_t_rad_t_electron = float(link_t_rad_t_electron)
+        p.delta_treatment = np.nan if delta_treatment is None else float(delta_treatment)
+        p.departure_coefficient = np.nan if departure_coefficient is None else float(departure_coefficient)
+        p.ion_zero_threshold = float(ion_zero_threshold)
+        keep = [t, w]
+        if electron_densities is not None:
+            ne = _f64(electron_densities)
+            if ne.shape != (S,):
+                raise ValueError(f"electron_densities needs one entry per shell ({S})")
+            keep.append(ne)
+            p.electron_densities = _dptr(ne)
+        it = C.c_int32(0)
+        out = None
+        if download:
+            n_levels, n_ions = self._plasma_shape
+            out = dict(electron_densities=np.empty(S), ion_number_density=np.empty((n_ions, S)),
+                       level_number_density=np.empty((n_levels, S)), j_blues=np.empty((L, S)))
+        ptr = (lambda k: _dptr(out[k])) if download else (lambda k: None)
+        self._check(self._api("solve_plasma")(self._h, C.byref(p), ptr("electron_densities"), ptr("ion_number_density"),
+                                              ptr("level_number_density"), ptr("j_blues"), C.byref(it)))
+        if out is None:
+            return dict(iterations=int(it.value))
+        out["iterations"] = int(it.value)
+        return out
 
     def download_opacity(self, transition_probabilities=False):
         """The device-built tables in the reference's host layout: dict of tau_sobolev, beta_sobolev,
@@ -697,6 +790,7 @@ class _MemberEngine(Engine):
         self._n_packets = 0
         self._n_continua = 0
         self._n_markov = 0
+        self._plasma_shape = None
         self._keep = []
 
     def close(self):
@@ -723,6 +817,7 @@ class EngineGroup(Engine):
         self._n_packets = 0
         self._n_continua = 0
         self._n_markov = 0
+        self._plasma_shape = None
         self._keep = []
         self.last_exact = None  # whether the last collective summed the fixed-point line accumulators
         for i, d in enumerate(devices):
@@ -766,6 +861,11 @@ class EngineGroup(Engine):
 
     def download_opacity(self, transition_probabilities=False):
         return self.members[0].download_opacity(transition_probabilities)
+
+    def set_plasma_data(self, **kw):
+        super().set_plasma_data(**kw)
+        for m in self.members:
+            m._plasma_shape = self._plasma_shape
 
     def build_absorbing_markov(self, *args, **kw):
         """On every member (`tb200_group_build_absorbing_markov`); the members' tables are bit-identical."""

@@ -715,3 +715,50 @@ def make_continuum_rate_inputs(n_shells: int, n_h_levels: int = 8, n_he_levels: 
             r[k][:, 0] = 0.0 if it == 0 else r[k][:, 0]   # a zero cooling channel in the first iteration
         rates.append(r)
     return ContinuumRateInputs(levels, lines, photoionization_data, ionization_energies, atomic, plasma, rates)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Inputs of the classic plasma (tb200_solve_plasma): an ion structure over make_atomic_data's levels
+# ---------------------------------------------------------------------------------------------------------------------
+EV_ERG = 1.602176565e-12  # CODATA-2010 (tardis/constants.py:1)
+
+
+@dataclass
+class PlasmaStructure:
+    """Ions over the levels of an AtomicData, in the reference's frame order: elements in ascending atomic number, each with
+    its ions of charge 0 ... Z (the bare ion included, as atomic data carry it), each ion a contiguous block of levels.
+    `ionization_energy` is ionization_data of (Z, charge): the energy into the ion (NaN for charge 0)."""
+
+    level_energy: np.ndarray       # f64[n_levels] erg: excitation energy (0 for the first level of every ion)
+    level_ion: np.ndarray          # i64[n_levels] row of the level's ion
+    ion_atomic_number: np.ndarray  # i64[n_ions]
+    ion_charge: np.ndarray         # i64[n_ions]
+    ionization_energy: np.ndarray  # f64[n_ions] erg
+    number_density: np.ndarray     # f64[n_elements, S] cm^-3
+    zeta_temperatures: np.ndarray  # f64[n_T] K
+    zeta: np.ndarray               # f64[n_ions, n_T]
+
+
+def make_plasma_structure(atomic: AtomicData, n_shells: int, atomic_numbers=tuple(range(1, 31)), seed: int = MODEL_SEED + 11,
+                          log_density: tuple[float, float] = (3.0, 9.0)) -> PlasmaStructure:
+    """Every ion gets at least one level and the rest of the levels are dealt out at random, in order.  A level's excitation
+    energy is its `atomic.energy` above the first level of its ion.  Ionisation energies grow with the charge (5-15 eV times
+    charge ** 1.3), so highly charged ions have Phi = 0 and populations below the zero threshold; zeta is U(0.05, 0.95) on a
+    2000-40000 K grid."""
+    rng = np.random.default_rng(seed)
+    zs = np.asarray(atomic_numbers, dtype=np.int64)
+    ion_z = np.concatenate([np.full(z + 1, z) for z in zs]).astype(np.int64)
+    ion_q = np.concatenate([np.arange(z + 1) for z in zs]).astype(np.int64)
+    n_ions, n = len(ion_z), atomic.n_levels
+    if n < n_ions:
+        raise ValueError(f"{n} levels cannot give {n_ions} ions one level each")
+    per_ion = 1 + rng.multinomial(n - n_ions, np.full(n_ions, 1.0 / n_ions))
+    level_ion = np.repeat(np.arange(n_ions, dtype=np.int64), per_ion)
+    first = np.concatenate([[0], np.cumsum(per_ion)[:-1]])
+    level_energy = atomic.energy - atomic.energy[first][level_ion]
+    chi = rng.uniform(5.0, 15.0, n_ions) * np.maximum(ion_q, 1) ** 1.3 * EV_ERG
+    chi[ion_q == 0] = np.nan
+    nd = 10 ** rng.uniform(*log_density, (len(zs), n_shells))
+    grid = np.arange(2000.0, 40001.0, 2000.0)
+    zeta = rng.uniform(0.05, 0.95, (n_ions, len(grid)))
+    return PlasmaStructure(np.ascontiguousarray(level_energy), level_ion, ion_z, ion_q, chi, np.ascontiguousarray(nd), grid, zeta)
